@@ -17,8 +17,10 @@
  *     allocation, no synchronisation, CUDA-graph capturable.  Calls marked
  *     [sync] synchronise the stream and may (re)allocate context scratch.
  *   - a context belongs to one device and is not thread-safe.
- *   - arithmetic is fp32 ("precision: single" in torchmd), energies are
- *     accumulated and returned in fp64.
+ *   - arithmetic is fp32 ("precision: single" in torchmd) by default, energies
+ *     are accumulated and returned in fp64.  A context set to 64 bits
+ *     (tmd_set_precision) runs "precision: double": fp64 state, parameters and
+ *     arithmetic through the *_f64 entry points, full neighbour rows, one GPU.
  */
 #ifndef TMD_B200_H
 #define TMD_B200_H
@@ -222,6 +224,48 @@ int tmd_wrapper_wrap(tmd_wrapper* w, float* pos_dev, const float* box_dev, int n
                      tmd_stream stream);
 int tmd_wrapper_destroy(tmd_wrapper* w);
 
+/* ---- "precision: double" ---------------------------------------------------------
+ *
+ * tmd_set_precision(ctx, 64) right after tmd_create, before any setter (TMD_ERR_STATE
+ * otherwise); the default is 32.  An fp64 context takes its parameters through the _f64
+ * setters below (tmd_set_exclusions, tmd_set_nonbonded and tmd_set_force_convention are
+ * shared) and its per-step work through the _f64 entry points, which mirror the fp32 ones
+ * with double state; an fp32 entry point on an fp64 context, or the reverse, returns
+ * TMD_ERR_STATE.  Neighbour decisions are the reference's fp64 chain bit for bit
+ * (d = p_i - p_j, w = d - L rint(d / L), sqrt_rn(fma(z,z,fma(y,y,x*x))) <= cutoff).  Full
+ * neighbour rows only; tmd_set_owned_atoms and tmd_dd_* return TMD_ERR_UNSUPPORTED.  With a
+ * cutoff, a coordinate of 8192 A or more from the origin is reported by tmd_get_stats
+ * (TMD_ERR_UNSUPPORTED: wrap the system) and a box length above 4096 A is refused
+ * (TMD_ERR_UNSUPPORTED at the first force call). */
+int tmd_set_precision(tmd_ctx* ctx, int bits);
+int tmd_set_atoms_f64(tmd_ctx* ctx, const double* charges_host, const int32_t* types_host,
+                      int ntypes, const double* A_host, const double* B_host);
+int tmd_set_bonds_f64(tmd_ctx* ctx, int n, const int32_t* idx_host, const double* prm_host);
+int tmd_set_angles_f64(tmd_ctx* ctx, int n, const int32_t* idx_host, const double* prm_host);
+int tmd_set_torsions_f64(tmd_ctx* ctx, int which, int n, const int32_t* idx_host,
+                         const int32_t* term_ptr_host, const double* terms_host, int amber_form);
+int tmd_set_pairs14_f64(tmd_ctx* ctx, int n, const int32_t* idx_host, const double* prm_host);
+int tmd_set_box_f64(tmd_ctx* ctx, const double* box_diag_host);
+int tmd_forces_f64(tmd_ctx* ctx, const double* pos_dev, double* forces_dev, double* energies_dev,
+                   tmd_stream stream);
+int tmd_vv_first_f64(tmd_ctx* ctx, double* pos_dev, double* vel_dev, const double* forces_dev,
+                     const double* masses_dev, double dt, tmd_stream stream);
+/* noise_dev NULL: fp64 normals from the Philox4x32-10 stream of tmd_vv_second (seed, step, atom) */
+int tmd_vv_second_f64(tmd_ctx* ctx, double* vel_dev, const double* forces_dev, const double* masses_dev,
+                      double dt, double gamma, const double* vcoeff_dev, const double* noise_dev,
+                      uint64_t seed, uint64_t step_index, double* ke_dev, tmd_stream stream);
+int tmd_kinetic_energy_f64(tmd_ctx* ctx, const double* vel_dev, const double* masses_dev, double* ke_dev,
+                           tmd_stream stream);
+/* niter steps enqueued with no host synchronisation (eager launches, no graph). */
+int tmd_md_steps_f64(tmd_ctx* ctx, int niter, double* pos_dev, double* vel_dev, double* forces_dev,
+                     const double* masses_dev, double dt, double gamma, const double* vcoeff_dev,
+                     const double* noise_dev, uint64_t seed, uint64_t first_step_index,
+                     double* energies_dev, double* ke_dev, tmd_stream stream);
+int tmd_export_pairs_f64(tmd_ctx* ctx, const double* pos_dev, int replica, int32_t* pairs_dev,
+                         int64_t capacity, int64_t* count_dev, tmd_stream stream);
+int tmd_wrapper_wrap_f64(tmd_wrapper* w, double* pos_dev, const double* box_dev, int nreplicas,
+                         tmd_stream stream);
+
 /* ---- inspection ------------------------------------------------------------ */
 
 /* The reference's neighbour list for one replica: every non-excluded pair
@@ -233,7 +277,8 @@ int tmd_export_pairs(tmd_ctx* ctx, const float* pos_dev, int replica, int32_t* p
 
 /* Which pair kernel the last tmd_forces / tmd_md_steps launched: 0 k_pair (float separations, the
  * default), 1 k_pair_fx (fixed-point separations), 2 k_pair_fx2 (fixed point + fp32x2
- * arithmetic), 3 k_pair2_open (no box, fp32x2 arithmetic).  For tests and bench labels. */
+ * arithmetic), 3 k_pair2_open (no box, fp32x2 arithmetic), 4 k_cpair (cluster lists),
+ * 5 k_pair_f64 (fp64 context).  For tests and bench labels. */
 int tmd_pair_kernel(tmd_ctx* ctx);
 
 typedef struct {

@@ -86,6 +86,21 @@ _SIGNATURES = {
     "tmd_wrapper_destroy": (C.c_int, [_P]),
     "tmd_profile_begin": (C.c_int, [_P, C.c_int]),
     "tmd_profile_end": (C.c_int, [_P, C.POINTER(C.c_double), C.POINTER(C.c_int), _P]),
+    # "precision: double" (library version >= 101)
+    "tmd_set_precision": (C.c_int, [_P, C.c_int]),
+    "tmd_set_atoms_f64": (C.c_int, [_P, _P, _P, C.c_int, _P, _P]),
+    "tmd_set_bonds_f64": (C.c_int, [_P, C.c_int, _P, _P]),
+    "tmd_set_angles_f64": (C.c_int, [_P, C.c_int, _P, _P]),
+    "tmd_set_torsions_f64": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P, C.c_int]),
+    "tmd_set_pairs14_f64": (C.c_int, [_P, C.c_int, _P, _P]),
+    "tmd_set_box_f64": (C.c_int, [_P, _P]),
+    "tmd_forces_f64": (C.c_int, [_P, _P, _P, _P, _P]),
+    "tmd_vv_first_f64": (C.c_int, [_P, _P, _P, _P, _P, C.c_double, _P]),
+    "tmd_vv_second_f64": (C.c_int, [_P, _P, _P, _P, C.c_double, C.c_double, _P, _P, C.c_uint64, C.c_uint64, _P, _P]),
+    "tmd_kinetic_energy_f64": (C.c_int, [_P, _P, _P, _P, _P]),
+    "tmd_md_steps_f64": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_double, C.c_double, _P, _P, C.c_uint64, C.c_uint64, _P, _P, _P]),
+    "tmd_export_pairs_f64": (C.c_int, [_P, _P, C.c_int, _P, C.c_int64, _P, _P]),
+    "tmd_wrapper_wrap_f64": (C.c_int, [_P, _P, _P, C.c_int, _P]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 
@@ -112,6 +127,8 @@ def lib():
                 f"{LIB_PATH} is the host SIMT-interpreter build of the kernels (tests/simt, a unit-test tool): "
                 "torchmd_b200 runs on the CUDA library only"
             )
+        if handle.tmd_version() < 101:
+            raise ImportError(f"{LIB_PATH} predates the fp64 entry points: rebuild it (__graft_entry__.build())")
         _lib = handle
     return _lib
 

@@ -113,13 +113,39 @@ struct DeviceState {
   ClusterState cl;
 };
 
-struct BondedSet {
+// P: type of the parameter rows, float ("precision: single") or double ("precision: double")
+template <typename P>
+struct BondedSetT {
   int n = 0;
   int* idx = nullptr;    // (n,k)
-  float* prm = nullptr;  // (n,p)
+  P* prm = nullptr;      // (n,p)
   int* term_ptr = nullptr;  // torsions only
-  float* terms = nullptr;
+  P* terms = nullptr;
   int amber = 1;
+};
+using BondedSet = BondedSetT<float>;
+
+// ---- "precision: double" (tmd_set_precision(ctx, 64)): full Verlet rows, fp64 state ------------
+// The list build is the fp32 one, run on an fp32 shadow of the positions (the list is a superset
+// of the pairs and decides nothing); the decision and every value are fp64.
+struct alignas(32) Rec64 {
+  double x, y, z, q;  // position + charge * sqrt(coulomb constant)
+};
+struct PairParams64 {
+  uint32_t terms;
+  int has_cutoff, has_switch, rfa, true_gradient;
+  double s_max;        // largest double s with sqrt_rn(s) <= cutoff; +inf without cutoff
+  double cutoff, switch_dist, inv_sw_width;  // 1 / (cutoff - switch_dist)
+  double krf, crf;     // reaction-field constants (forces.py:466-468)
+};
+struct DeviceState64 {
+  Rec64* xq_s;         // [rep*(natoms+1) + k] sorted records; record natoms is the NaN sentinel
+  float* shadow;       // (R,N,3) positions rounded to fp32: what the list build reads
+  const double* q;     // charge * sqrt(coulomb constant)
+  const double* AB;    // (T*T) {A,B} interleaved
+  const double* L;     // (R,3) box lengths
+  double pos_limit;    // |coordinate| from which F_FARPOS is raised (the shadow's rounding must stay inside the list margin)
+  PairParams64 pp;
 };
 
 }  // namespace tmd
@@ -169,4 +195,15 @@ struct tmd_ctx {
   int64_t force_calls = 0;
   double* ke_scratch = nullptr;      // (nrep) doubles for the host entry
   double* e_scratch = nullptr;       // (nrep, TMD_NUM_ENERGIES)
+  // "precision: double" (tmd_set_precision)
+  int precision = 32;
+  bool touched = false;              // a setter has run: the precision is fixed
+  tmd::DeviceState64 d64{};
+  tmd::Rec64* xq64 = nullptr;        // owned buffers behind d64
+  float* shadow = nullptr;
+  double* q64 = nullptr;
+  double* AB64 = nullptr;
+  double* L64 = nullptr;
+  std::vector<double> charges64_host, box64_host;
+  tmd::BondedSetT<double> bonds64, angles64, torsions64[2], pairs1464;
 };

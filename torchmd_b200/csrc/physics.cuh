@@ -173,10 +173,80 @@ TMD_HD bool ref_inside(float xi, float yi, float zi, float xj, float yj, float z
   return norm2_ref(wx, wy, wz) <= s_max;
 }
 
+// ---- fp64 decision arithmetic ("precision: double") -------------------------------------
+// The reference's fp64 path makes the same decision with the same rounded operations in
+// double: w = d - L * rint(d / L) (four separately rounded ops), s = fma(z,z,fma(y,y,x*x))
+// (torch.norm(dim=1) on (P,3) fp64, bit-identical on x86-64), inside iff sqrt_rn(s) <= cutoff.
+// The overloads keep nvcc from contracting any of it.
+TMD_HD double mul_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+  return __dmul_rn(a, b);
+#else
+  volatile double r = a * b;
+  return r;
+#endif
+}
+TMD_HD double add_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+  return __dadd_rn(a, b);
+#else
+  volatile double r = a + b;
+  return r;
+#endif
+}
+TMD_HD double sub_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+  return __dsub_rn(a, b);
+#else
+  volatile double r = a - b;
+  return r;
+#endif
+}
+TMD_HD double div_rn(double a, double b) {
+#if defined(__CUDA_ARCH__)
+  return __ddiv_rn(a, b);
+#else
+  volatile double r = a / b;
+  return r;
+#endif
+}
+TMD_HD double fma_rn(double a, double b, double c) {
+#if defined(__CUDA_ARCH__)
+  return __fma_rn(a, b, c);
+#else
+  return fma(a, b, c);
+#endif
+}
+TMD_HD double sqrt_rn(double a) {
+#if defined(__CUDA_ARCH__)
+  return __dsqrt_rn(a);
+#else
+  volatile double r = sqrt(a);
+  return r;
+#endif
+}
+// Minimum image of one fp64 component, the reference's rounding for any separation.
+TMD_HD double min_image64(double d, double L) { return sub_rn(d, mul_rn(L, rint(div_rn(d, L)))); }
+TMD_HD double norm2_ref(double x, double y, double z) { return fma_rn(z, z, fma_rn(y, y, mul_rn(x, x))); }
+// Largest double s with sqrt_rn(s) <= rc (host only): the fp64 decision on the squared distance.
+inline double squared_threshold64(double rc) {
+  double s = rc * rc;
+  while (sqrt(s) > rc) s = nextafter(s, 0.0);
+  for (;;) {
+    const double up = nextafter(s, INFINITY);
+    if (sqrt(up) <= rc) s = up;
+    else break;
+  }
+  return s;
+}
+
 // ---- Wrapper.wrap (wrapper.py:24-27): image offset of a group from its coordinate sum ----
 //   com = sum / len ;  offset = floor(com / box) * box        (three rounded fp32 operations)
 TMD_HD float wrap_offset(float coord_sum, int len, float box) {
   return mul_rn(floorf(div_rn(div_rn(coord_sum, (float)len), box)), box);
+}
+TMD_HD double wrap_offset(double coord_sum, int len, double box) {
+  return mul_rn(floor(div_rn(div_rn(coord_sum, (double)len), box)), box);
 }
 
 // ---- fixed-point periodic coordinates ---------------------------------------------------

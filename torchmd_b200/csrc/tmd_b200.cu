@@ -21,6 +21,7 @@
 #include "pair.cuh"
 #include "cluster.cuh"
 #include "fused.cuh"
+#include "double.cuh"
 
 using namespace tmd;
 
@@ -210,6 +211,14 @@ struct tmd_ctx_full : tmd_ctx {
   CtxPriv priv;
 };
 static inline CtxPriv& priv(tmd_ctx* c) { return static_cast<tmd_ctx_full*>(c)->priv; }
+// An fp32 entry point on an fp64 context (or the reverse) is a call-order error.
+static int need_precision(tmd_ctx* ctx, int bits, const char* name) {
+  if (ctx->precision == bits) return TMD_OK;
+  return fail(TMD_ERR_STATE, std::string(name) + ": this context runs in " + (ctx->precision == 64 ? "fp64" : "fp32") +
+                                 " (tmd_set_precision); use the " + (ctx->precision == 64 ? "_f64" : "fp32") + " entry point");
+}
+#define TMD_PRECISION(ctx, bits, name) \
+  if (int rc__ = need_precision((ctx), (bits), (name))) return rc__;
 // ---- peer-to-peer position exchange --------------------------------------------------------
 static inline float* dd_pos_of(tmd_ctx* ctx, int peer, int which) {
   return reinterpret_cast<float*>(static_cast<char*>(ctx->dd_peer_base[peer]) + (size_t)which * ctx->dd_pos_bytes);
@@ -235,7 +244,7 @@ const char* tmd_last_error(void) { return g_err.c_str(); }
 #if defined(TMD_SIMT_HOST)
 int tmd_version(void) { return -100; }  // host SIMT interpreter build (tests/simt): torchmd_b200/_lib.py refuses it
 #else
-int tmd_version(void) { return 100; }
+int tmd_version(void) { return 101; }  // 101: the "precision: double" entry points (tmd_set_precision, *_f64)
 #endif
 
 int tmd_create(tmd_ctx** out, int device, int natoms, int nreplicas) {
@@ -294,7 +303,12 @@ int tmd_destroy(tmd_ctx* ctx) {
                   ctx->bonds.idx, ctx->bonds.prm, ctx->angles.idx, ctx->angles.prm,
                   ctx->torsions[0].idx, ctx->torsions[0].term_ptr, ctx->torsions[0].terms,
                   ctx->torsions[1].idx, ctx->torsions[1].term_ptr, ctx->torsions[1].terms,
-                  ctx->pairs14.idx, ctx->pairs14.prm, ctx->bonded_atom_ptr, ctx->bonded_entries, ctx->xf_buf};
+                  ctx->pairs14.idx, ctx->pairs14.prm, ctx->bonded_atom_ptr, ctx->bonded_entries, ctx->xf_buf,
+                  ctx->xq64, ctx->shadow, ctx->q64, ctx->AB64, ctx->L64,
+                  ctx->bonds64.idx, ctx->bonds64.prm, ctx->angles64.idx, ctx->angles64.prm,
+                  ctx->torsions64[0].idx, ctx->torsions64[0].term_ptr, ctx->torsions64[0].terms,
+                  ctx->torsions64[1].idx, ctx->torsions64[1].term_ptr, ctx->torsions64[1].terms,
+                  ctx->pairs1464.idx, ctx->pairs1464.prm};
   for (void* b : bufs)
     if (b) cudaFree(b);
   dd_release(ctx);
@@ -320,6 +334,7 @@ int tmd_destroy(tmd_ctx* ctx) {
 int tmd_set_atoms(tmd_ctx* ctx, const float* charges, const int32_t* types, int ntypes,
                   const float* A, const float* B) {
   if (!ctx || !charges || !types || ntypes <= 0) return fail(TMD_ERR_ARG, "tmd_set_atoms: bad arguments");
+  TMD_PRECISION(ctx, 32, "tmd_set_atoms")
   DeviceGuard guard(ctx->device);
   for (int i = 0; i < ctx->natoms; ++i)
     if (types[i] < 0 || types[i] >= ntypes) return fail(TMD_ERR_ARG, "tmd_set_atoms: atom type out of range");
@@ -332,6 +347,7 @@ int tmd_set_atoms(tmd_ctx* ctx, const float* charges, const int32_t* types, int 
   if ((rc = upload(&ctx->AB, ab.data(), ab.size()))) return rc;
   ctx->d.ntypes = ntypes;
   ctx->have_atoms = true;
+  ctx->touched = true;
   priv(ctx).dirty = true;
   return TMD_OK;
 }
@@ -349,6 +365,7 @@ int tmd_set_exclusions(tmd_ctx* ctx, const int64_t* row_ptr, const int32_t* cols
   if ((rc = upload(&ctx->excl_ptr, rp.data(), rp.size()))) return rc;
   if ((rc = upload(&ctx->excl_idx, cols, (size_t)row_ptr[n]))) return rc;
   ctx->have_excl = row_ptr[n] > 0;
+  ctx->touched = true;
   priv(ctx).dirty = true;
   return TMD_OK;
 }
@@ -387,13 +404,34 @@ int tmd_set_nonbonded(tmd_ctx* ctx, uint32_t term_mask, double cutoff, double sw
     pp.crf = (float)crf;
     pp.two_krf = (float)(2.0 * krf);
   }
+  {  // the same set-up for the fp64 kernels (contexts of tmd_set_precision(ctx, 64))
+    PairParams64& p = ctx->d64.pp;
+    memset(&p, 0, sizeof(p));
+    p.terms = ctx->pair_mask;
+    p.has_cutoff = cutoff >= 0;
+    p.cutoff = p.has_cutoff ? cutoff : INFINITY;
+    p.s_max = p.has_cutoff ? squared_threshold64(cutoff) : INFINITY;
+    p.has_switch = pp.has_switch;
+    p.switch_dist = p.has_switch ? switch_dist : 0.0;
+    p.inv_sw_width = p.has_switch ? 1.0 / (cutoff - switch_dist) : 1.0;
+    p.rfa = pp.rfa;
+    if (rfa) {
+      const double denom = 2.0 * solvent_dielectric + 1.0;
+      p.krf = (1.0 / (cutoff * cutoff * cutoff)) * (solvent_dielectric - 1.0) / denom;
+      p.crf = (1.0 / cutoff) * (3.0 * solvent_dielectric) / denom;
+    }
+    p.true_gradient = ctx->exact_gradient;
+  }
   ctx->have_nonbonded = true;
+  ctx->touched = true;
   priv(ctx).dirty = true;
   return TMD_OK;
 }
 
-static int set_bonded(tmd_ctx* ctx, BondedSet& s, std::vector<int32_t>& idx_h, int n, int k, int p,
-                      const int32_t* idx, const float* prm) {
+extern "C++" {  // (templates inside the C-linkage block)
+template <typename P>
+static int set_bonded(tmd_ctx* ctx, BondedSetT<P>& s, std::vector<int32_t>& idx_h, int n, int k, int p,
+                      const int32_t* idx, const P* prm) {
   DeviceGuard guard(ctx->device);
   if (n < 0 || (n > 0 && (!idx || !prm))) return fail(TMD_ERR_ARG, "bonded set: bad arguments");
   for (long long e = 0; e < (long long)n * k; ++e)
@@ -403,27 +441,32 @@ static int set_bonded(tmd_ctx* ctx, BondedSet& s, std::vector<int32_t>& idx_h, i
   if ((rc = upload(&s.prm, prm, (size_t)n * p))) return rc;
   s.n = n;
   idx_h.assign(idx, idx + (size_t)n * k);
+  ctx->touched = true;
   priv(ctx).dirty = true;
   return TMD_OK;
 }
+}  // extern "C++"
 
 int tmd_set_bonds(tmd_ctx* ctx, int n, const int32_t* idx, const float* prm) {
   if (!ctx) return fail(TMD_ERR_ARG, "null context");
+  TMD_PRECISION(ctx, 32, "tmd_set_bonds")
   return set_bonded(ctx, ctx->bonds, ctx->bonds_idx_h, n, 2, 2, idx, prm);
 }
 int tmd_set_angles(tmd_ctx* ctx, int n, const int32_t* idx, const float* prm) {
   if (!ctx) return fail(TMD_ERR_ARG, "null context");
+  TMD_PRECISION(ctx, 32, "tmd_set_angles")
   return set_bonded(ctx, ctx->angles, ctx->angles_idx_h, n, 3, 2, idx, prm);
 }
 int tmd_set_pairs14(tmd_ctx* ctx, int n, const int32_t* idx, const float* prm) {
   if (!ctx) return fail(TMD_ERR_ARG, "null context");
+  TMD_PRECISION(ctx, 32, "tmd_set_pairs14")
   return set_bonded(ctx, ctx->pairs14, ctx->pairs14_idx_h, n, 2, 4, idx, prm);
 }
-int tmd_set_torsions(tmd_ctx* ctx, int which, int n, const int32_t* idx, const int32_t* term_ptr,
-                     const float* terms, int amber_form) {
-  if (!ctx || which < 0 || which > 1) return fail(TMD_ERR_ARG, "tmd_set_torsions: bad arguments");
+extern "C++" {  // (templates inside the C-linkage block)
+template <typename P>
+static int set_torsions(tmd_ctx* ctx, BondedSetT<P>& s, int which, int n, const int32_t* idx, const int32_t* term_ptr,
+                        const P* terms, int amber_form) {
   DeviceGuard guard(ctx->device);
-  BondedSet& s = ctx->torsions[which];
   if (n < 0 || (n > 0 && (!idx || !term_ptr || !terms))) return fail(TMD_ERR_ARG, "tmd_set_torsions: bad arguments");
   for (long long e = 0; e < (long long)n * 4; ++e)
     if (idx[e] < 0 || idx[e] >= ctx->natoms) return fail(TMD_ERR_ARG, "tmd_set_torsions: atom index out of range");
@@ -434,29 +477,109 @@ int tmd_set_torsions(tmd_ctx* ctx, int which, int n, const int32_t* idx, const i
   s.n = n;
   s.amber = amber_form ? 1 : 0;
   ctx->torsions_idx_h[which].assign(idx, idx + (size_t)n * 4);
+  ctx->touched = true;
   priv(ctx).dirty = true;
   return TMD_OK;
 }
+}  // extern "C++"
+int tmd_set_torsions(tmd_ctx* ctx, int which, int n, const int32_t* idx, const int32_t* term_ptr,
+                     const float* terms, int amber_form) {
+  if (!ctx || which < 0 || which > 1) return fail(TMD_ERR_ARG, "tmd_set_torsions: bad arguments");
+  TMD_PRECISION(ctx, 32, "tmd_set_torsions")
+  return set_torsions(ctx, ctx->torsions[which], which, n, idx, term_ptr, terms, amber_form);
+}
 
-int tmd_set_box(tmd_ctx* ctx, const float* box_diag) {
-  if (!ctx || !box_diag) return fail(TMD_ERR_ARG, "tmd_set_box: bad arguments");
+// ---- "precision: double" --------------------------------------------------------------------
+int tmd_set_precision(tmd_ctx* ctx, int bits) {
+  if (!ctx || (bits != 32 && bits != 64)) return fail(TMD_ERR_ARG, "tmd_set_precision: 32 or 64");
+  if (ctx->touched || ctx->force_calls || ctx->launches)
+    return fail(TMD_ERR_STATE, "tmd_set_precision: call it right after tmd_create, before any setter");
+  ctx->precision = bits;
+  return TMD_OK;
+}
+
+int tmd_set_atoms_f64(tmd_ctx* ctx, const double* charges, const int32_t* types, int ntypes, const double* A,
+                      const double* B) {
+  if (!ctx || !charges || !types || ntypes <= 0) return fail(TMD_ERR_ARG, "tmd_set_atoms_f64: bad arguments");
+  TMD_PRECISION(ctx, 64, "tmd_set_atoms_f64")
+  DeviceGuard guard(ctx->device);
+  for (int i = 0; i < ctx->natoms; ++i)
+    if (types[i] < 0 || types[i] >= ntypes) return fail(TMD_ERR_ARG, "tmd_set_atoms_f64: atom type out of range");
+  ctx->charges64_host.assign(charges, charges + ctx->natoms);
+  ctx->charges_host.assign(charges, charges + ctx->natoms);  // (the fp32 records of the list build)
+  int rc;
+  if ((rc = upload(&ctx->type, types, (size_t)ctx->natoms))) return rc;
+  std::vector<float2> ab((size_t)ntypes * ntypes, make_float2(0.f, 0.f));
+  std::vector<double> ab64(2 * ab.size(), 0.0);
+  if (A && B)
+    for (size_t t = 0; t < ab.size(); ++t) {
+      ab64[2 * t] = A[t];
+      ab64[2 * t + 1] = B[t];
+    }
+  if ((rc = upload(&ctx->AB, ab.data(), ab.size()))) return rc;
+  if ((rc = upload(&ctx->AB64, ab64.data(), ab64.size()))) return rc;
+  ctx->d.ntypes = ntypes;
+  ctx->have_atoms = true;
+  ctx->touched = true;
+  priv(ctx).dirty = true;
+  return TMD_OK;
+}
+int tmd_set_bonds_f64(tmd_ctx* ctx, int n, const int32_t* idx, const double* prm) {
+  if (!ctx) return fail(TMD_ERR_ARG, "null context");
+  TMD_PRECISION(ctx, 64, "tmd_set_bonds_f64")
+  return set_bonded(ctx, ctx->bonds64, ctx->bonds_idx_h, n, 2, 2, idx, prm);
+}
+int tmd_set_angles_f64(tmd_ctx* ctx, int n, const int32_t* idx, const double* prm) {
+  if (!ctx) return fail(TMD_ERR_ARG, "null context");
+  TMD_PRECISION(ctx, 64, "tmd_set_angles_f64")
+  return set_bonded(ctx, ctx->angles64, ctx->angles_idx_h, n, 3, 2, idx, prm);
+}
+int tmd_set_pairs14_f64(tmd_ctx* ctx, int n, const int32_t* idx, const double* prm) {
+  if (!ctx) return fail(TMD_ERR_ARG, "null context");
+  TMD_PRECISION(ctx, 64, "tmd_set_pairs14_f64")
+  return set_bonded(ctx, ctx->pairs1464, ctx->pairs14_idx_h, n, 2, 4, idx, prm);
+}
+int tmd_set_torsions_f64(tmd_ctx* ctx, int which, int n, const int32_t* idx, const int32_t* term_ptr,
+                         const double* terms, int amber_form) {
+  if (!ctx || which < 0 || which > 1) return fail(TMD_ERR_ARG, "tmd_set_torsions_f64: bad arguments");
+  TMD_PRECISION(ctx, 64, "tmd_set_torsions_f64")
+  return set_torsions(ctx, ctx->torsions64[which], which, n, idx, term_ptr, terms, amber_form);
+}
+
+extern "C++" {  // (templates inside the C-linkage block)
+template <typename T>
+static int set_box(tmd_ctx* ctx, const T* box_diag) {
   int nzero = 0;
   for (int e = 0; e < ctx->nrep * 3; ++e) {
-    if (!(box_diag[e] >= 0.f)) return fail(TMD_ERR_ARG, "tmd_set_box: negative or NaN box length");
-    nzero += (box_diag[e] == 0.f);
+    if (!(box_diag[e] >= T(0))) return fail(TMD_ERR_ARG, "tmd_set_box: negative or NaN box length");
+    nzero += (box_diag[e] == T(0));
   }
   if (nzero != 0 && nzero != ctx->nrep * 3)
     return fail(TMD_ERR_UNSUPPORTED, "tmd_set_box: box must be all zero (no wrapping) or all positive");
   ctx->periodic = (nzero == 0);
   ctx->box_host.assign(box_diag, box_diag + ctx->nrep * 3);
+  ctx->box64_host.assign(box_diag, box_diag + ctx->nrep * 3);
   ctx->have_box = true;
+  ctx->touched = true;
   priv(ctx).dirty = true;
   return TMD_OK;
+}
+}  // extern "C++"
+int tmd_set_box(tmd_ctx* ctx, const float* box_diag) {
+  if (!ctx || !box_diag) return fail(TMD_ERR_ARG, "tmd_set_box: bad arguments");
+  TMD_PRECISION(ctx, 32, "tmd_set_box")
+  return set_box(ctx, box_diag);
+}
+int tmd_set_box_f64(tmd_ctx* ctx, const double* box_diag) {
+  if (!ctx || !box_diag) return fail(TMD_ERR_ARG, "tmd_set_box_f64: bad arguments");
+  TMD_PRECISION(ctx, 64, "tmd_set_box_f64")
+  return set_box(ctx, box_diag);
 }
 
 }  // extern "C"
 
 // ---- finalise: host-side sizing, allocation, uploads (first use / after changes) ----------
+static constexpr double F64_POS_LIMIT = 8192.0;  // A: fp64 contexts flag coordinates from here on (margin, finalize)
 static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   if (!ctx->have_atoms) return fail(TMD_ERR_STATE, "tmd_set_atoms has not been called");
   if (!ctx->have_box) return fail(TMD_ERR_STATE, "tmd_set_box has not been called");
@@ -480,7 +603,28 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   d.excl_idx = ctx->have_excl ? ctx->excl_idx : nullptr;
 
   const bool has_cut = ctx->cutoff >= 0;
-  const double margin = 0.004;  // A: fp32 slack of the approximate build arithmetic and of binning
+  const bool f64 = ctx->precision == 64;
+  // fp64 contexts build the list from an fp32 shadow of the positions (double.cuh), so the list radius also covers
+  // what that shadow can be off by.  Conditions: every |coordinate| < P = F64_POS_LIMIT = 2^13 A (else k_prepare_f64
+  // raises F_FARPOS, which tmd_get_stats reports) and every box length L <= 2^12 A (else refused below).  Below 2^13 an
+  // fp32 ulp is at most 2^-11 A; h = 2^-12 A is half of it.  Per coordinate of one atom, against the exact fp64 geometry,
+  // the build sees at most:
+  //   the shadow's rounding                                                    h
+  //   the fold x - L*floor(x/L) of phase_sort_pack, product and subtraction
+  //   rounded separately (no contraction assumed): |L*floor(x/L)| < P + L
+  //   <= 1.5 * 2^13, half an ulp 2h; the result is below 2L <= 2^13:           2h + h
+  //   fp32 box length against the fp64 one, |floor(x/L)| * |L32 - L64|
+  //   <= (P/L + 1) * L * 2^-24 = (P + L) * 2^-24 <= 1.5 * 2^-11:               3h
+  // so 7h per atom, and per component of a pair 14h plus h for the one image shift the build adds with L32 (|L32 - L64|
+  // <= h): 15h, sqrt(3) * 15h < 26h on a distance.  The displacement trigger compares shadows with shadows; an atom's
+  // true displacement exceeds its shadow displacement by at most 2 sqrt(3) h, a pair's distance by 4 sqrt(3) h < 7h.
+  // With the fp32 slack of the build arithmetic and binning (0.004 A) the radius needs 26h + 7h = 33h more; 36h =
+  // 0.0088 A is added.
+  const double margin = 0.004 + (f64 ? 36.0 / 4096.0 : 0.0);  // A
+  if (f64 && ctx->periodic)
+    for (int e = 0; e < R * 3; ++e)
+      if (ctx->box_host[e] > 4096.f)
+        return fail(TMD_ERR_UNSUPPORTED, "fp64 contexts take box lengths up to 4096 A (the fp32 shadow of the list build)");
   const double rl = has_cut ? ctx->cutoff + ctx->skin + margin : INFINITY;
   d.rlist = (float)rl;
   d.rlist2 = has_cut ? (float)(rl * rl) : INFINITY;
@@ -491,7 +635,7 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   // can hold must have ONE image within reach (size condition below).  Otherwise: full Verlet rows.
   ClusterState& cl = d.cl;
   const double cl_extent = 8.0;  // a periodic box must leave room for clusters at least this long (A)
-  bool use_cluster = env_switch("TMD_B200_CLUSTER", TMD_DEFAULT_CLUSTER) == 1 && !ctx->cluster_failed && has_cut &&
+  bool use_cluster = env_switch("TMD_B200_CLUSTER", TMD_DEFAULT_CLUSTER) == 1 && !f64 && !ctx->cluster_failed && has_cut &&
                      ctx->pair_mask != 0 && (ctx->pair_mask & ~(T_LJ | T_ELEC)) == 0 && !ctx->exact_gradient &&
                      d.ntypes <= CL_MAXT && N < (1 << 24) - 4096 * CL;
   double cl_max_extent = INFINITY;
@@ -566,7 +710,7 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   {
     const int fx = env_switch("TMD_B200_FX", TMD_DEFAULT_FX);
     ctx->fx_packed = fx == 2;
-    if ((((fx == 1 || fx == 2) && ctx->safe_image) || (use_cluster && ctx->periodic)) && ctx->pair_mask) {
+    if ((((fx == 1 || fx == 2) && ctx->safe_image) || (use_cluster && ctx->periodic)) && ctx->pair_mask && !f64) {
       if (!use_cluster) {
         const size_t n = (size_t)R * N + R;
         if ((rc = device_alloc(&ctx->xf_buf, n))) return rc;
@@ -745,7 +889,7 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
     if ((rc = upload(&ctx->bonded_atom_ptr, ptr.data(), ptr.size()))) return rc;
     if ((rc = upload(&ctx->bonded_entries, ent.data(), ent.size()))) return rc;
     CtxPriv& pv = priv(ctx);
-    pv.bonded_terms = env_switch("TMD_B200_BONDED_TERMS", 1) == 1;
+    pv.bonded_terms = env_switch("TMD_B200_BONDED_TERMS", 1) == 1 || f64;  // (fp64: the two-pass kernels only)
     const size_t need = pv.bonded_terms ? (size_t)R * ptr[N] * 3 : 0;  // one slot per (term, atom of the term) = per entry
     if (need > pv.term_forces_len) {
       if (pv.term_forces) cudaFree(pv.term_forces);
@@ -772,7 +916,7 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   // bonded kernel concurrent with the pair kernel (TMD_B200_OVERLAP)
   {
     CtxPriv& pv = priv(ctx);
-    const bool want = env_switch("TMD_B200_OVERLAP", TMD_DEFAULT_OVERLAP) == 1 && ctx->bonded_nentries > 0 && ctx->pair_mask;
+    const bool want = env_switch("TMD_B200_OVERLAP", TMD_DEFAULT_OVERLAP) == 1 && ctx->bonded_nentries > 0 && ctx->pair_mask && !f64;
     if (want && !pv.side) {
       TMD_CUDA(cudaStreamCreateWithFlags(&pv.side, cudaStreamNonBlocking));
       TMD_CUDA(cudaEventCreateWithFlags(&pv.ev_fork, cudaEventDisableTiming));
@@ -799,6 +943,24 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
     pv.fuse_prepare = env_switch("TMD_B200_FUSEPREP", TMD_DEFAULT_FUSEPREP) == 1;
     pv.fuse_step = env_switch("TMD_B200_FUSESTEP", TMD_DEFAULT_FUSESTEP) == 1;
     pv.steps_valid = false;  // buffers may have moved: captured steps are rebuilt
+  }
+  if (f64) {
+    DeviceState64& D = ctx->d64;
+    std::vector<double> qs(N);
+    const double sk = sqrt(ctx->coulomb > 0 ? ctx->coulomb : 0.0);
+    for (int i = 0; i < N; ++i) qs[i] = ctx->charges64_host[i] * sk;
+    if ((rc = upload(&ctx->q64, qs.data(), (size_t)N))) return rc;
+    if ((rc = upload(&ctx->L64, ctx->box64_host.data(), ctx->box64_host.size()))) return rc;
+    if ((rc = device_alloc(&ctx->xq64, (size_t)R * (N + 1)))) return rc;
+    TMD_CUDA(cudaMemset(ctx->xq64, 0xFF, (size_t)R * (N + 1) * sizeof(Rec64)));  // NaN, incl. the sentinels
+    if ((rc = device_alloc(&ctx->shadow, (size_t)R * N * 3))) return rc;
+    D.xq_s = ctx->xq64;
+    D.shadow = ctx->shadow;
+    D.q = ctx->q64;
+    D.AB = ctx->AB64;
+    D.L = ctx->L64;
+    D.pos_limit = has_cut ? F64_POS_LIMIT : INFINITY;  // without a cutoff every pair is listed: nothing to bound
+    D.pp.true_gradient = ctx->exact_gradient;
   }
   priv(ctx).dirty = false;
   return TMD_OK;
@@ -867,6 +1029,113 @@ static inline dim3 owned_grid(const tmd_ctx* ctx, int threads) {
   return dim3((unsigned)((std::max(ctx->d.own_n, 1) + threads - 1) / threads), (unsigned)ctx->nrep);
 }
 
+// The kernels' bonded table (BondedTables or BondedTables64) from the context's sets, disabled terms emptied.
+template <typename Tables, typename Set>
+static Tables bonded_tables(const tmd_ctx* ctx, const Set& bonds, const Set& angles, const Set* torsions, const Set& pairs14) {
+  const uint32_t bm = ctx->bonded_mask;
+  Tables T;
+  T.atom_ptr = ctx->bonded_atom_ptr;
+  T.entries = ctx->bonded_entries;
+  T.bonds = bonds;
+  T.angles = angles;
+  T.torsions[0] = torsions[0];
+  T.torsions[1] = torsions[1];
+  T.pairs14 = pairs14;
+  if (!(bm & TMD_TERM(TMD_E_BONDS))) T.bonds.n = 0;
+  if (!(bm & TMD_TERM(TMD_E_ANGLES))) T.angles.n = 0;
+  if (!(bm & TMD_TERM(TMD_E_DIHEDRALS))) T.torsions[0].n = 0;
+  if (!(bm & TMD_TERM(TMD_E_IMPROPERS))) T.torsions[1].n = 0;
+  if (!(bm & TMD_TERM(TMD_E_14))) T.pairs14.n = 0;
+  return T;
+}
+// Where each (kind, term, slot) force sits in the per-term buffer of k_bonded_terms / k_bonded_sum.
+template <typename Tables>
+static TermLayout term_layout(const Tables& T) {
+  TermLayout lay;
+  const int cnt[5] = {T.bonds.n, T.angles.n, T.torsions[0].n, T.torsions[1].n, T.pairs14.n};
+  int nt = 0, ns = 0;
+  for (int k = 0; k < 5; ++k) {
+    lay.first[k] = nt;
+    lay.slot0[k] = ns;
+    nt += cnt[k];
+    ns += cnt[k] * term_arity(k);
+  }
+  lay.nterms = nt;
+  lay.nslots = ns;
+  return lay;
+}
+
+// The gated full-row rebuild (neighbor.cuh) from the fp32 positions `pos`: every kernel returns at once unless
+// k_prepare raised the replica's rebuild flag.
+static int enqueue_rebuild_rows(tmd_ctx* ctx, const float* pos, int need_bounds, cudaStream_t rs) {
+  const DeviceState& d = ctx->d;
+  const int R = ctx->nrep;
+  if (need_bounds) {
+    launch(k_bounds, atoms_grid(ctx, 256), 256, rs, d, pos);
+    TMD_LAUNCHED(ctx, "k_bounds");
+    launch(k_grid, (R + 63) / 64, 64, rs, d);
+    TMD_LAUNCHED(ctx, "k_grid");
+  }
+  launch(k_bin, atoms_grid(ctx, 256), 256, rs, d, pos);
+  TMD_LAUNCHED(ctx, "k_bin");
+  launch(k_scan, R, 1024, rs, d);
+  TMD_LAUNCHED(ctx, "k_scan");
+  launch(k_place, atoms_grid(ctx, 256), 256, rs, d);
+  TMD_LAUNCHED(ctx, "k_place");
+  {
+    const int blocks = std::max(1, std::min((d.max_cells + 7) / 8, ctx->nsm * 8));
+    launch(k_sort_pack, dim3(blocks, R), 256, rs, d);
+    TMD_LAUNCHED(ctx, "k_sort_pack");
+  }
+  launch(k_build_list, dim3(std::max(1, std::min(d.max_cells * std::max(1, d.build_split), ctx->nsm * 12)), R), BT_WARPS * 32, rs, d);
+  TMD_LAUNCHED(ctx, "k_build_list");
+  return TMD_OK;
+}
+
+// Forces.compute on an fp64 context: preparation (fp32 shadow), the gated fp32 list build on the shadow, the fp64
+// records in the new order, k_pair_f64, then the two bonded passes in stream order.
+static int enqueue_forces_f64(tmd_ctx* ctx, const double* pos, double* forces, double* energies, cudaStream_t st) {
+  const DeviceState& d = ctx->d;
+  const DeviceState64& D = ctx->d64;
+  const int N = ctx->natoms, R = ctx->nrep;
+  ctx->force_calls++;
+  if (energies) TMD_CUDA(cudaMemsetAsync(energies, 0, (size_t)R * TMD_NUM_ENERGIES * sizeof(double), st));
+  if (ctx->pair_mask) {
+    launch(k_prepare_f64, atoms_grid(ctx, 256), 256, st, d, D, pos);
+    TMD_LAUNCHED(ctx, "k_prepare_f64");
+    if (int rc = enqueue_rebuild_rows(ctx, D.shadow, (!ctx->periodic && ctx->cutoff >= 0) ? 1 : 0, st)) return rc;
+    launch(k_pack_f64, atoms_grid(ctx, 256), 256, st, d, D, pos);
+    TMD_LAUNCHED(ctx, "k_pack_f64");
+    CtxPriv& pv = priv(ctx);
+    const bool sample = pv.profiling && (size_t)(pv.ev_used + 2) <= pv.ev.size();
+    if (sample) TMD_CUDA(cudaEventRecord(pv.ev[pv.ev_used], st));
+    const dim3 pg((N + PAIR_WARPS - 1) / PAIR_WARPS, R);
+    const int th = PAIR_WARPS * 32;
+    ctx->last_pair_kernel = 5;
+    if (energies && ctx->periodic) launch(k_pair_f64<true, true>, pg, th, st, d, D, forces, energies);
+    else if (energies) launch(k_pair_f64<true, false>, pg, th, st, d, D, forces, energies);
+    else if (ctx->periodic) launch(k_pair_f64<false, true>, pg, th, st, d, D, forces, energies);
+    else launch(k_pair_f64<false, false>, pg, th, st, d, D, forces, energies);
+    TMD_LAUNCHED(ctx, "k_pair_f64");
+    if (sample) {
+      TMD_CUDA(cudaEventRecord(pv.ev[pv.ev_used + 1], st));
+      pv.ev_used += 2;
+    }
+  } else {
+    TMD_CUDA(cudaMemsetAsync(forces, 0, (size_t)R * N * 3 * sizeof(double), st));
+  }
+  if (ctx->bonded_nentries > 0) {
+    const BondedTables64 T = bonded_tables<BondedTables64>(ctx, ctx->bonds64, ctx->angles64, ctx->torsions64, ctx->pairs1464);
+    const TermLayout lay = term_layout(T);
+    launch(k_bonded_terms_f64, dim3((std::max(lay.nterms, 1) + BONDED_THREADS - 1) / BONDED_THREADS, R), BONDED_THREADS, st, d, D, T, lay,
+           pos, energies, priv(ctx).term_forces);
+    TMD_LAUNCHED(ctx, "k_bonded_terms_f64");
+    launch(k_bonded_sum_f64, atoms_grid(ctx, BONDED_THREADS), BONDED_THREADS, st, d, T, lay, (const double*)priv(ctx).term_forces, forces);
+    TMD_LAUNCHED(ctx, "k_bonded_sum_f64");
+  }
+  return TMD_OK;
+}
+
 static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double* energies, cudaStream_t st) {
   DeviceState& d = ctx->d;
   const int N = ctx->natoms, R = ctx->nrep;
@@ -875,21 +1144,7 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
 
   BondedTables T;
   const bool have_bonded = ctx->bonded_nentries > 0;
-  if (have_bonded) {
-    const uint32_t bm = ctx->bonded_mask;
-    T.atom_ptr = ctx->bonded_atom_ptr;
-    T.entries = ctx->bonded_entries;
-    T.bonds = ctx->bonds;
-    T.angles = ctx->angles;
-    T.torsions[0] = ctx->torsions[0];
-    T.torsions[1] = ctx->torsions[1];
-    T.pairs14 = ctx->pairs14;
-    if (!(bm & TMD_TERM(TMD_E_BONDS))) T.bonds.n = 0;
-    if (!(bm & TMD_TERM(TMD_E_ANGLES))) T.angles.n = 0;
-    if (!(bm & TMD_TERM(TMD_E_DIHEDRALS))) T.torsions[0].n = 0;
-    if (!(bm & TMD_TERM(TMD_E_IMPROPERS))) T.torsions[1].n = 0;
-    if (!(bm & TMD_TERM(TMD_E_14))) T.pairs14.n = 0;
-  }
+  if (have_bonded) T = bonded_tables<BondedTables>(ctx, ctx->bonds, ctx->angles, ctx->torsions, ctx->pairs14);
   // bonded forces of the owned atoms: terms in parallel, then the fixed-order sum per atom (bonded.cuh)
   auto launch_bonded = [&](cudaStream_t bs, double* scratch) -> int {
     CtxPriv& pv = priv(ctx);
@@ -898,18 +1153,8 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
       TMD_LAUNCHED(ctx, "k_bonded");
       return TMD_OK;
     }
-    TermLayout lay;
-    const int cnt[5] = {T.bonds.n, T.angles.n, T.torsions[0].n, T.torsions[1].n, T.pairs14.n};
-    int nt = 0, ns = 0;
-    for (int k = 0; k < 5; ++k) {
-      lay.first[k] = nt;
-      lay.slot0[k] = ns;
-      nt += cnt[k];
-      ns += cnt[k] * term_arity(k);
-    }
-    lay.nterms = nt;
-    lay.nslots = ns;
-    launch(k_bonded_terms, dim3((std::max(nt, 1) + BONDED_THREADS - 1) / BONDED_THREADS, R), BONDED_THREADS, bs, d, T, lay, ctx->q, pos,
+    const TermLayout lay = term_layout(T);
+    launch(k_bonded_terms, dim3((std::max(lay.nterms, 1) + BONDED_THREADS - 1) / BONDED_THREADS, R), BONDED_THREADS, bs, d, T, lay, ctx->q, pos,
            energies, pv.term_forces);
     TMD_LAUNCHED(ctx, "k_bonded_terms");
     launch(k_bonded_sum, owned_grid(ctx, BONDED_THREADS), BONDED_THREADS, bs, d, T, lay, pv.term_forces, forces, scratch);
@@ -998,25 +1243,7 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
                                            args, 0, st));
       TMD_LAUNCHED(ctx, "k_rebuild");
     } else {
-      if (need_bounds) {
-        launch(k_bounds, atoms_grid(ctx, 256), 256, rs, d, pos);
-        TMD_LAUNCHED(ctx, "k_bounds");
-        launch(k_grid, (R + 63) / 64, 64, rs, d);
-        TMD_LAUNCHED(ctx, "k_grid");
-      }
-      launch(k_bin, atoms_grid(ctx, 256), 256, rs, d, pos);
-      TMD_LAUNCHED(ctx, "k_bin");
-      launch(k_scan, R, 1024, rs, d);
-      TMD_LAUNCHED(ctx, "k_scan");
-      launch(k_place, atoms_grid(ctx, 256), 256, rs, d);
-      TMD_LAUNCHED(ctx, "k_place");
-      {
-        const int blocks = std::max(1, std::min((d.max_cells + 7) / 8, ctx->nsm * 8));
-        launch(k_sort_pack, dim3(blocks, R), 256, rs, d);
-        TMD_LAUNCHED(ctx, "k_sort_pack");
-      }
-      launch(k_build_list, dim3(std::max(1, std::min(d.max_cells * std::max(1, d.build_split), ctx->nsm * 12)), R), BT_WARPS * 32, rs, d);
-      TMD_LAUNCHED(ctx, "k_build_list");
+      if (int brc = enqueue_rebuild_rows(ctx, pos, need_bounds, rs)) return brc;
     }
     if (in_body) {
       priv(ctx).last_body_launches = ctx->launches - body_l0;
@@ -1189,6 +1416,7 @@ extern "C" {
 
 int tmd_forces(tmd_ctx* ctx, const float* pos, float* forces, double* energies, tmd_stream stream) {
   if (!ctx || !pos || !forces) return fail(TMD_ERR_ARG, "tmd_forces: null pointer");
+  TMD_PRECISION(ctx, 32, "tmd_forces")
   DeviceGuard guard(ctx->device);
   cudaStream_t st = (cudaStream_t)stream;
   int rc;
@@ -1200,6 +1428,7 @@ int tmd_forces(tmd_ctx* ctx, const float* pos, float* forces, double* energies, 
 int tmd_vv_first(tmd_ctx* ctx, float* pos, float* vel, const float* forces, const float* masses, double dt,
                  tmd_stream stream) {
   if (!ctx || !pos || !vel || !forces || !masses) return fail(TMD_ERR_ARG, "tmd_vv_first: null pointer");
+  TMD_PRECISION(ctx, 32, "tmd_vv_first")
   DeviceGuard guard(ctx->device);
   return enqueue_vv_first(ctx, pos, vel, forces, masses, dt, (cudaStream_t)stream);
 }
@@ -1208,6 +1437,7 @@ int tmd_vv_second(tmd_ctx* ctx, float* vel, const float* forces, const float* ma
                   const float* vcoeff, const float* noise, uint64_t seed, uint64_t step_index, double* ke,
                   tmd_stream stream) {
   if (!ctx || !vel || !forces || !masses) return fail(TMD_ERR_ARG, "tmd_vv_second: null pointer");
+  TMD_PRECISION(ctx, 32, "tmd_vv_second")
   DeviceGuard guard(ctx->device);
   return enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step_index, ke,
                            (cudaStream_t)stream);
@@ -1215,6 +1445,7 @@ int tmd_vv_second(tmd_ctx* ctx, float* vel, const float* forces, const float* ma
 
 int tmd_kinetic_energy(tmd_ctx* ctx, const float* vel, const float* masses, double* ke, tmd_stream stream) {
   if (!ctx || !vel || !masses || !ke) return fail(TMD_ERR_ARG, "tmd_kinetic_energy: null pointer");
+  TMD_PRECISION(ctx, 32, "tmd_kinetic_energy")
   DeviceGuard guard(ctx->device);
   cudaStream_t st = (cudaStream_t)stream;
   TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
@@ -1227,6 +1458,7 @@ int tmd_md_steps(tmd_ctx* ctx, int niter, float* pos, float* vel, float* forces,
                  double dt, double gamma, const float* vcoeff, const float* noise, uint64_t seed,
                  uint64_t first_step, double* energies, double* ke, tmd_stream stream) {
   if (!ctx || !pos || !vel || !forces || !masses || niter < 0) return fail(TMD_ERR_ARG, "tmd_md_steps: bad arguments");
+  TMD_PRECISION(ctx, 32, "tmd_md_steps")
   DeviceGuard guard(ctx->device);
   cudaStream_t st = (cudaStream_t)stream;
   int rc;
@@ -1333,6 +1565,7 @@ int tmd_md_steps_host(tmd_ctx* ctx, int niter, float* pos_host, float* vel_host,
                       const float* vcoeff_dev, uint64_t seed, uint64_t first_step, double* energies_host,
                       double* ke_host, tmd_stream stream) {
   if (!ctx || !pos_host || !vel_host || !pos_dev || !vel_dev) return fail(TMD_ERR_ARG, "tmd_md_steps_host: null pointer");
+  TMD_PRECISION(ctx, 32, "tmd_md_steps_host")
   DeviceGuard guard(ctx->device);
   cudaStream_t st = (cudaStream_t)stream;
   const size_t bytes = (size_t)ctx->nrep * ctx->natoms * 3 * sizeof(float);
@@ -1352,10 +1585,118 @@ int tmd_md_steps_host(tmd_ctx* ctx, int niter, float* pos_host, float* vel_host,
   return TMD_OK;
 }
 
+// ---- "precision: double" per-step entry points ---------------------------------------------
+int tmd_forces_f64(tmd_ctx* ctx, const double* pos, double* forces, double* energies, tmd_stream stream) {
+  if (!ctx || !pos || !forces) return fail(TMD_ERR_ARG, "tmd_forces_f64: null pointer");
+  TMD_PRECISION(ctx, 64, "tmd_forces_f64")
+  DeviceGuard guard(ctx->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  if (priv(ctx).dirty && (rc = finalize(ctx, st))) return rc;
+  return enqueue_forces_f64(ctx, pos, forces, energies, st);
+}
+
+static void enqueue_vv_first_f64(tmd_ctx* ctx, double* pos, double* vel, const double* forces, const double* masses, double dt,
+                                 cudaStream_t st) {
+  launch(k_vv_first_f64, atoms_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, ctx->natoms, ctx->d.counters, pos, vel, forces, masses,
+         dt, 0.5 * dt);
+}
+static void enqueue_vv_second_f64(tmd_ctx* ctx, double* vel, const double* forces, const double* masses, double dt, double gamma,
+                                  const double* vcoeff, const double* noise, uint64_t seed, uint64_t step, double* ke,
+                                  cudaStream_t st) {
+  const bool thermo = (gamma >= 0.0) && vcoeff != nullptr;
+  const dim3 g = atoms_grid(ctx, INTEG_THREADS);
+  const int n = ctx->natoms;
+  const unsigned long long* ctr = ctx->d.counters;
+  if (thermo) {
+    if (ke) launch(k_vv_second_f64<true, true>, g, INTEG_THREADS, st, n, ctr, vel, forces, masses, dt, 0.5 * dt, -gamma, vcoeff, noise, seed, step, ke);
+    else launch(k_vv_second_f64<true, false>, g, INTEG_THREADS, st, n, ctr, vel, forces, masses, dt, 0.5 * dt, -gamma, vcoeff, noise, seed, step, ke);
+  } else {
+    if (ke) launch(k_vv_second_f64<false, true>, g, INTEG_THREADS, st, n, ctr, vel, forces, masses, dt, 0.5 * dt, -gamma, vcoeff, noise, seed, step, ke);
+    else launch(k_vv_second_f64<false, false>, g, INTEG_THREADS, st, n, ctr, vel, forces, masses, dt, 0.5 * dt, -gamma, vcoeff, noise, seed, step, ke);
+  }
+}
+
+int tmd_vv_first_f64(tmd_ctx* ctx, double* pos, double* vel, const double* forces, const double* masses, double dt,
+                     tmd_stream stream) {
+  if (!ctx || !pos || !vel || !forces || !masses) return fail(TMD_ERR_ARG, "tmd_vv_first_f64: null pointer");
+  TMD_PRECISION(ctx, 64, "tmd_vv_first_f64")
+  DeviceGuard guard(ctx->device);
+  enqueue_vv_first_f64(ctx, pos, vel, forces, masses, dt, (cudaStream_t)stream);
+  TMD_LAUNCHED(ctx, "k_vv_first_f64");
+  return TMD_OK;
+}
+
+int tmd_vv_second_f64(tmd_ctx* ctx, double* vel, const double* forces, const double* masses, double dt, double gamma,
+                      const double* vcoeff, const double* noise, uint64_t seed, uint64_t step_index, double* ke,
+                      tmd_stream stream) {
+  if (!ctx || !vel || !forces || !masses) return fail(TMD_ERR_ARG, "tmd_vv_second_f64: null pointer");
+  TMD_PRECISION(ctx, 64, "tmd_vv_second_f64")
+  DeviceGuard guard(ctx->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (ke) TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
+  enqueue_vv_second_f64(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step_index, ke, st);
+  TMD_LAUNCHED(ctx, "k_vv_second_f64");
+  return TMD_OK;
+}
+
+int tmd_kinetic_energy_f64(tmd_ctx* ctx, const double* vel, const double* masses, double* ke, tmd_stream stream) {
+  if (!ctx || !vel || !masses || !ke) return fail(TMD_ERR_ARG, "tmd_kinetic_energy_f64: null pointer");
+  TMD_PRECISION(ctx, 64, "tmd_kinetic_energy_f64")
+  DeviceGuard guard(ctx->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
+  launch(k_kinetic_f64, atoms_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, ctx->natoms, vel, masses, ke);
+  TMD_LAUNCHED(ctx, "k_kinetic_f64");
+  return TMD_OK;
+}
+
+int tmd_md_steps_f64(tmd_ctx* ctx, int niter, double* pos, double* vel, double* forces, const double* masses, double dt,
+                     double gamma, const double* vcoeff, const double* noise, uint64_t seed, uint64_t first_step,
+                     double* energies, double* ke, tmd_stream stream) {
+  if (!ctx || !pos || !vel || !forces || !masses || niter < 0) return fail(TMD_ERR_ARG, "tmd_md_steps_f64: bad arguments");
+  TMD_PRECISION(ctx, 64, "tmd_md_steps_f64")
+  DeviceGuard guard(ctx->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  if (priv(ctx).dirty && (rc = finalize(ctx, st))) return rc;
+  const size_t per_step = (size_t)ctx->nrep * ctx->natoms * 3;
+  for (int it = 0; it < niter; ++it) {
+    const bool last = (it == niter - 1);
+    enqueue_vv_first_f64(ctx, pos, vel, forces, masses, dt, st);
+    TMD_LAUNCHED(ctx, "k_vv_first_f64");
+    if ((rc = enqueue_forces_f64(ctx, pos, forces, last ? energies : nullptr, st))) return rc;
+    if (last && ke) TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
+    enqueue_vv_second_f64(ctx, vel, forces, masses, dt, gamma, vcoeff, noise ? noise + it * per_step : nullptr, seed, first_step,
+                          last ? ke : nullptr, st);
+    TMD_LAUNCHED(ctx, "k_vv_second_f64");
+  }
+  return TMD_OK;
+}
+
+int tmd_export_pairs_f64(tmd_ctx* ctx, const double* pos, int replica, int32_t* pairs, int64_t capacity, int64_t* count,
+                         tmd_stream stream) {
+  if (!ctx || !pairs || !count || replica < 0 || replica >= ctx->nrep)
+    return fail(TMD_ERR_ARG, "tmd_export_pairs_f64: bad arguments");
+  TMD_PRECISION(ctx, 64, "tmd_export_pairs_f64")
+  if (!ctx->pair_mask) return fail(TMD_ERR_STATE, "tmd_export_pairs_f64: no pair term enabled");
+  if (priv(ctx).dirty || ctx->force_calls == 0)
+    return fail(TMD_ERR_STATE, "tmd_export_pairs_f64: call tmd_forces_f64 on these positions first");
+  (void)pos;
+  DeviceGuard guard(ctx->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  TMD_CUDA(cudaMemsetAsync(count, 0, sizeof(int64_t), st));
+  launch(k_export_pairs_f64, (ctx->natoms + 3) / 4, 128, st, ctx->d, ctx->d64, replica, pairs, (long long)capacity,
+         reinterpret_cast<unsigned long long*>(count));
+  TMD_LAUNCHED(ctx, "k_export_pairs_f64");
+  return TMD_OK;
+}
+
 int tmd_export_pairs(tmd_ctx* ctx, const float* pos, int replica, int32_t* pairs, int64_t capacity,
                      int64_t* count, tmd_stream stream) {
   if (!ctx || !pairs || !count || replica < 0 || replica >= ctx->nrep)
     return fail(TMD_ERR_ARG, "tmd_export_pairs: bad arguments");
+  TMD_PRECISION(ctx, 32, "tmd_export_pairs")
   if (!ctx->pair_mask) return fail(TMD_ERR_STATE, "tmd_export_pairs: no pair term enabled");
   if (priv(ctx).dirty || ctx->force_calls == 0)
     return fail(TMD_ERR_STATE, "tmd_export_pairs: call tmd_forces on these positions first");
@@ -1379,6 +1720,7 @@ int tmd_set_force_convention(tmd_ctx* ctx, int exact_gradient) {
   if (!ctx) return fail(TMD_ERR_ARG, "tmd_set_force_convention: null context");
   ctx->exact_gradient = exact_gradient ? 1 : 0;
   ctx->d.pp.true_gradient = ctx->exact_gradient;  // uniform kernel parameter: takes effect at the next launch
+  ctx->d64.pp.true_gradient = ctx->exact_gradient;
   ctx->pair_mode = (ctx->pair_mask == (T_LJ | T_ELEC) && ctx->d.pp.has_switch && ctx->d.pp.rfa && !ctx->exact_gradient) ? 1 : 0;
   return TMD_OK;
 }
@@ -1386,6 +1728,7 @@ int tmd_set_force_convention(tmd_ctx* ctx, int exact_gradient) {
 int tmd_set_owned_atoms(tmd_ctx* ctx, int first_atom, int count) {
   if (!ctx || first_atom < 0 || count < 0 || first_atom + count > ctx->natoms)
     return fail(TMD_ERR_ARG, "tmd_set_owned_atoms: range outside the system");
+  if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_owned_atoms: fp64 contexts run the whole system on one GPU");
   ctx->d.own_lo = first_atom;
   ctx->d.own_n = count;
   ctx->d.own_all = (first_atom == 0 && count == ctx->natoms) ? 1 : 0;
@@ -1397,6 +1740,7 @@ int tmd_set_owned_atoms(tmd_ctx* ctx, int first_atom, int count) {
 int tmd_dd_create(tmd_ctx* ctx, int rank, int world, unsigned char* handle_out) {
   if (!ctx || !handle_out || world < 1 || world > TMD_MAX_PEERS || rank < 0 || rank >= world)
     return fail(TMD_ERR_ARG, "tmd_dd_create: bad arguments (at most 16 ranks)");
+  if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_create: fp64 contexts run the whole system on one GPU");
   if (ctx->nrep != 1) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_create: decomposed runs take one replica");
   static_assert(sizeof(cudaIpcMemHandle_t) == TMD_IPC_HANDLE_BYTES, "IPC handle size");
   DeviceGuard guard(ctx->device);
@@ -1419,6 +1763,7 @@ int tmd_dd_create(tmd_ctx* ctx, int rank, int world, unsigned char* handle_out) 
 
 int tmd_dd_connect(tmd_ctx* ctx, const unsigned char* handles) {
   if (!ctx || !handles) return fail(TMD_ERR_ARG, "tmd_dd_connect: null pointer");
+  if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_connect: fp64 contexts run the whole system on one GPU");
   if (!ctx->dd_base) return fail(TMD_ERR_STATE, "tmd_dd_connect: tmd_dd_create has not been called");
   DeviceGuard guard(ctx->device);
   for (int p = 0; p < ctx->dd_world; ++p) {
@@ -1435,6 +1780,7 @@ int tmd_dd_connect(tmd_ctx* ctx, const unsigned char* handles) {
 
 #define TMD_DD_READY(name)                                                                     \
   if (!ctx) return fail(TMD_ERR_ARG, name ": null context");                                   \
+  if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, name ": fp64 contexts run the whole system on one GPU"); \
   if (!ctx->dd_connected) return fail(TMD_ERR_STATE, name ": tmd_dd_create / tmd_dd_connect first"); \
   DeviceGuard guard(ctx->device);
 
@@ -1523,17 +1869,26 @@ int tmd_wrapper_create(tmd_wrapper** out, int device, int natoms, int ngroups, c
   return TMD_OK;
 }
 
-int tmd_wrapper_wrap(tmd_wrapper* w, float* pos, const float* box, int nrep, tmd_stream stream) {
+extern "C++" {  // (templates inside the C-linkage block)
+template <typename T>
+static int wrapper_wrap(tmd_wrapper* w, T* pos, const T* box, int nrep, tmd_stream stream) {
   if (!w || !pos || !box || nrep <= 0 || nrep > 65535) return fail(TMD_ERR_ARG, "tmd_wrapper_wrap: bad arguments");
   if (w->ngroups == 0) return TMD_OK;
   DeviceGuard guard(w->device);
   cudaStream_t st = (cudaStream_t)stream;
-  launch(k_wrap_boxflag, 1, 256, st, box, nrep, w->flag);
-  launch(k_wrap, dim3((unsigned)((w->ngroups + WRAP_WARPS - 1) / WRAP_WARPS), (unsigned)nrep), WRAP_WARPS * 32, st, 
+  launch(k_wrap_boxflag<T>, 1, 256, st, box, nrep, w->flag);
+  launch(k_wrap<T>, dim3((unsigned)((w->ngroups + WRAP_WARPS - 1) / WRAP_WARPS), (unsigned)nrep), WRAP_WARPS * 32, st, 
       w->natoms, w->ngroups, w->group_ptr, w->group_atoms, pos, box, w->flag);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(TMD_ERR_CUDA, std::string("launch k_wrap: ") + cudaGetErrorString(e));
   return TMD_OK;
+}
+}  // extern "C++"
+int tmd_wrapper_wrap(tmd_wrapper* w, float* pos, const float* box, int nrep, tmd_stream stream) {
+  return wrapper_wrap(w, pos, box, nrep, stream);
+}
+int tmd_wrapper_wrap_f64(tmd_wrapper* w, double* pos, const double* box, int nrep, tmd_stream stream) {
+  return wrapper_wrap(w, pos, box, nrep, stream);
 }
 
 int tmd_wrapper_destroy(tmd_wrapper* w) {
@@ -1607,8 +1962,11 @@ int tmd_get_stats(tmd_ctx* ctx, tmd_stats* out, tmd_stream stream) {
   for (int r = 0; r < ctx->nrep; ++r)
     if (fl[r * F_COUNT + F_FARPOS])
       return fail(TMD_ERR_UNSUPPORTED,
-                  "a position is more than 2000 box lengths from the origin: wrap the coordinates "
-                  "(torchmd Wrapper) -- results since the last check are not reliable");
+                  ctx->precision == 64
+                      ? "a position is 8192 A or more from the origin (fp64 contexts), or not finite: wrap the coordinates "
+                        "(torchmd Wrapper) -- results since the last check are not reliable"
+                      : "a position is more than 2000 box lengths from the origin: wrap the coordinates "
+                        "(torchmd Wrapper) -- results since the last check are not reliable");
   if (ctx->cluster_failed && ctx->force_calls >= ctx->cluster_retry_at && !priv(ctx).dirty) {
     ctx->cluster_failed = false;  // try the cluster lists again from the next force call on
     priv(ctx).dirty = true;

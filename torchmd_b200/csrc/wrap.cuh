@@ -19,16 +19,19 @@ namespace tmd {
 constexpr int WRAP_WARPS = 8;
 
 // flag[0] = 1 if every box length of every replica is zero (the reference returns at once)
-__global__ void k_wrap_boxflag(const float* __restrict__ box, int nrep, int* __restrict__ flag) {
+// T: float ("precision: single") or double ("precision: double"), the dtype of the positions and the box
+template <typename T>
+__global__ void k_wrap_boxflag(const T* __restrict__ box, int nrep, int* __restrict__ flag) {
   int nonzero = 0;
-  for (int e = threadIdx.x; e < nrep * 3; e += blockDim.x) nonzero |= (box[(e / 3) * 9 + (e % 3) * 4] != 0.f);
+  for (int e = threadIdx.x; e < nrep * 3; e += blockDim.x) nonzero |= (box[(e / 3) * 9 + (e % 3) * 4] != T(0));
   nonzero = __syncthreads_or(nonzero);
   if (threadIdx.x == 0) flag[0] = nonzero ? 0 : 1;
 }
 
+template <typename T>
 __global__ void __launch_bounds__(WRAP_WARPS * 32)
 k_wrap(int natoms, int ngroups, const int* __restrict__ group_ptr, const int* __restrict__ group_atoms,
-       float* __restrict__ pos, const float* __restrict__ box, const int* __restrict__ allzero) {
+       T* __restrict__ pos, const T* __restrict__ box, const int* __restrict__ allzero) {
   if (allzero[0]) return;
   const int lane = threadIdx.x & 31;
   const int g = blockIdx.x * WRAP_WARPS + (threadIdx.x >> 5);
@@ -36,11 +39,11 @@ k_wrap(int natoms, int ngroups, const int* __restrict__ group_ptr, const int* __
   if (g >= ngroups) return;
   const int b = group_ptr[g], n = group_ptr[g + 1] - b;
   if (n <= 0) return;
-  float* p = pos + (size_t)r * natoms * 3;
-  const float L[3] = {box[r * 9 + 0], box[r * 9 + 4], box[r * 9 + 8]};
-  float sum[3] = {0.f, 0.f, 0.f};
+  T* p = pos + (size_t)r * natoms * 3;
+  const T L[3] = {box[r * 9 + 0], box[r * 9 + 4], box[r * 9 + 8]};
+  T sum[3] = {T(0), T(0), T(0)};
   if (n <= 32) {
-    float v[3] = {0.f, 0.f, 0.f};
+    T v[3] = {T(0), T(0), T(0)};
     if (lane < n) {
       const size_t a = (size_t)group_atoms[b + lane] * 3;
       v[0] = p[a];
@@ -50,7 +53,7 @@ k_wrap(int natoms, int ngroups, const int* __restrict__ group_ptr, const int* __
     for (int m = 0; m < n; ++m) {  // every lane forms the same sequential sum
 #pragma unroll
       for (int d = 0; d < 3; ++d) {
-        const float t = __shfl_sync(0xffffffffu, v[d], m);
+        const T t = __shfl_sync(0xffffffffu, v[d], m);
         sum[d] = (m == 0) ? t : add_rn(sum[d], t);
       }
     }
@@ -64,7 +67,7 @@ k_wrap(int natoms, int ngroups, const int* __restrict__ group_ptr, const int* __
     for (int d = 0; d < 3; ++d)
       for (int o = 16; o; o >>= 1) sum[d] = add_rn(sum[d], __shfl_xor_sync(0xffffffffu, sum[d], o));
   }
-  float off[3];
+  T off[3];
 #pragma unroll
   for (int d = 0; d < 3; ++d) off[d] = wrap_offset(sum[d], n, L[d]);
   for (int e = lane; e < n; e += 32) {

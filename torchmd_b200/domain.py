@@ -86,6 +86,8 @@ class DecomposedIntegrator:
     """
 
     def __init__(self, system, forces, timestep, device, gamma=None, T=None, group=None, use_graph=True, exchange=None):
+        if system.pos.dtype == torch.float64:
+            raise NotImplementedError("decomposed runs are fp32 only: run 'precision: double' on one GPU")
         if system.pos.shape[0] != 1:
             raise NotImplementedError("decomposed runs take one replica; shard replicas across ranks instead")
         self.exchange = (exchange or os.environ.get("TMD_B200_EXCHANGE", "allgather")).lower()

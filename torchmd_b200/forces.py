@@ -9,8 +9,10 @@ unchanged.  Differences that are deliberate:
 * no O(N^2) pair table: exclusions go to the device as a CSR adjacency and the
   neighbour search is a cell list + Verlet list (``ava_idx`` is only
   materialised on request, for small systems);
-* ``pos`` / ``forces`` must be CUDA fp32 contiguous tensors -- there is no CPU or
-  stock-PyTorch fallback, a missing extension or a CPU tensor raises;
+* ``pos`` / ``forces`` must be CUDA contiguous tensors -- there is no CPU or
+  stock-PyTorch fallback, a missing extension or a CPU tensor raises.  Their dtype is the
+  run's precision: float32 ("precision: single") or float64 ("precision: double": fp64
+  parameters, arithmetic and neighbour decisions, full neighbour rows, one GPU);
 * energies are accumulated in fp64 on the device.
 """
 import os
@@ -139,11 +141,13 @@ class Forces:
             self._ava_idx = torch.tensor(np.argwhere(np.triu(ok, 1))).to(self.par.device)
         return self._ava_idx
 
-    def _check_tensor(self, t, name, shape=None):
+    def _check_tensor(self, t, name, shape=None, dtype=None):
         if not torch.is_tensor(t) or not _lib.on_device(t):
             raise RuntimeError(f"{name} must be a CUDA tensor: torchmd_b200 has no CPU path")
-        if t.dtype != torch.float32:
-            raise NotImplementedError(f"{name} must be float32 (precision: single); got {t.dtype}")
+        if t.dtype not in (torch.float32, torch.float64):
+            raise NotImplementedError(f"{name} must be float32 (precision: single) or float64 (precision: double); got {t.dtype}")
+        if dtype is not None and t.dtype != dtype:
+            raise RuntimeError(f"{name} is {t.dtype} but the positions are {dtype}: one precision per call")
         if not t.is_contiguous():
             raise RuntimeError(f"{name} must be contiguous")
         if shape is not None and tuple(t.shape) != tuple(shape):
@@ -152,7 +156,7 @@ class Forces:
     def _ensure_ctx(self, pos):
         """Create the device context on first use (needs the replica count and device)."""
         nrep = pos.shape[0]
-        key = (pos.device.index if pos.device.index is not None else torch.cuda.current_device(), nrep)
+        key = (pos.device.index if pos.device.index is not None else torch.cuda.current_device(), nrep, pos.dtype)
         if self._ctx is not None and self._ctx_key == key:
             return self._ctx
         L = _lib.lib()
@@ -166,16 +170,29 @@ class Forces:
         handle = C.c_void_p()
         _lib.check(L.tmd_create(C.byref(handle), key[0], self.natoms, nrep))
         ctx = handle
-        self._configure(L, ctx, _lib.check)
+        if pos.dtype == torch.float64:
+            try:
+                _lib.check(L.tmd_set_precision(ctx, 64))
+            except Exception:
+                L.tmd_destroy(ctx)
+                raise
+        self._configure(L, ctx, _lib.check, f64=pos.dtype == torch.float64)
         self._ctx, self._ctx_key, self._box_key, self._box_ref = ctx, key, None, None
         self._exact_gradient = False
         return ctx
 
-    def _configure(self, L, ctx, check):
+    def _configure(self, L, ctx, check, f64=False):
         """Hand topology and parameters to a fresh context (every tmd_set_* call; host data only).
-        ``L`` is the bound library, ``check`` raises on a non-zero return code."""
+        ``L`` is the bound library, ``check`` raises on a non-zero return code.  ``f64``: an fp64 context
+        (tmd_set_precision), whose parameters go over in fp64 through the ``_f64`` setters."""
         par = self.par
-        charges = _np(par.charges, np.float32)
+        real = np.float64 if f64 else np.float32
+        sfx = "_f64" if f64 else ""
+
+        def setter(name):
+            return getattr(L, name + sfx)
+
+        charges = _np(par.charges, real)
         if par.mapped_atom_types is not None:
             types = _np(par.mapped_atom_types, np.int32)
         else:
@@ -186,9 +203,9 @@ class Forces:
         if need_ab:
             if getattr(par, "A", None) is None:
                 par.A, par.B = par.get_AB()
-            A, B = _np(par.A, np.float32), _np(par.B, np.float32)
+            A, B = _np(par.A, real), _np(par.B, real)
             ntypes = A.shape[0]
-        check(L.tmd_set_atoms(ctx, _lib.ptr(charges), _lib.ptr(types), ntypes, _lib.ptr(A), _lib.ptr(B)))
+        check(setter("tmd_set_atoms")(ctx, _lib.ptr(charges), _lib.ptr(types), ntypes, _lib.ptr(A), _lib.ptr(B)))
 
         if self.require_distances:
             row_ptr, cols = _exclusion_csr(self.natoms, par.get_exclusions(self._exclusion_types))
@@ -211,16 +228,16 @@ class Forces:
             """Per-instance parameter rows: params[map[:,1]] ordered by map[:,0]."""
             idx = _np(term["idx"], np.int32)
             m = term["map"].detach().cpu().numpy()
-            prm = _np(term["params"], np.float32)[m[:, 1]]
+            prm = _np(term["params"], real)[m[:, 1]]
             order = np.argsort(m[:, 0], kind="stable")
             return idx, m[order, 0], np.ascontiguousarray(prm[order])
 
         if "bonds" in self.energies and par.bond_params is not None:
             idx, _, prm = instance_rows(par.bond_params)
-            check(L.tmd_set_bonds(ctx, len(idx), _lib.ptr(idx), _lib.ptr(prm)))
+            check(setter("tmd_set_bonds")(ctx, len(idx), _lib.ptr(idx), _lib.ptr(prm)))
         if "angles" in self.energies and par.angle_params is not None:
             idx, _, prm = instance_rows(par.angle_params)
-            check(L.tmd_set_angles(ctx, len(idx), _lib.ptr(idx), _lib.ptr(prm)))
+            check(setter("tmd_set_angles")(ctx, len(idx), _lib.ptr(idx), _lib.ptr(prm)))
         for which, name, term in (
             (0, "dihedrals", par.dihedral_params),
             (1, "impropers", par.improper_params),
@@ -231,21 +248,23 @@ class Forces:
                 term_ptr = np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
                 amber = bool(np.all(prm[:, 2] > 0))  # forces.py:566, decided over the whole set
                 check(
-                    L.tmd_set_torsions(ctx, which, len(idx), _lib.ptr(idx), _lib.ptr(term_ptr), _lib.ptr(prm), int(amber))
+                    setter("tmd_set_torsions")(ctx, which, len(idx), _lib.ptr(idx), _lib.ptr(term_ptr), _lib.ptr(prm), int(amber))
                 )
         if "1-4" in self.energies and par.nonbonded_14_params is not None and len(par.nonbonded_14_params["idx"]):
             idx, _, prm = instance_rows(par.nonbonded_14_params)
-            check(L.tmd_set_pairs14(ctx, len(idx), _lib.ptr(idx), _lib.ptr(prm)))
+            check(setter("tmd_set_pairs14")(ctx, len(idx), _lib.ptr(idx), _lib.ptr(prm)))
 
     def _ensure_box(self, box):
         """Hand the box diagonal to the context when the tensor changed (one D2H copy).  The tensor the
         key was taken from is kept alive: its storage cannot go back to the caching allocator, so a
         fresh box tensor can never reproduce the (address, version) of the one already uploaded."""
-        key = (box.data_ptr(), box._version, tuple(box.shape), tuple(box.stride()))
+        key = (box.data_ptr(), box._version, tuple(box.shape), tuple(box.stride()), box.dtype)
         if key == self._box_key and self._box_ref is not None:
             return
-        diag = np.ascontiguousarray(torch.diagonal(box, dim1=1, dim2=2).detach().cpu().numpy().astype(np.float32))
-        _lib.check(_lib.lib().tmd_set_box(self._ctx, _lib.ptr(diag)))
+        f64 = self._ctx_key[2] == torch.float64
+        diag = np.ascontiguousarray(torch.diagonal(box, dim1=1, dim2=2).detach().cpu().numpy().astype(np.float64 if f64 else np.float32))
+        L = _lib.lib()
+        _lib.check((L.tmd_set_box_f64 if f64 else L.tmd_set_box)(self._ctx, _lib.ptr(diag)))
         self._box_key, self._box_ref = key, box
 
     # ------------------------------------------------------------------ compute
@@ -259,9 +278,11 @@ class Forces:
         reference's autograd path yields) instead of its explicit formula (forces.py:410-412)."""
         self._check_tensor(pos, "pos")
         nrep = pos.shape[0]
-        self._check_tensor(forces, "forces", pos.shape)
+        self._check_tensor(forces, "forces", pos.shape, pos.dtype)
         if not torch.is_tensor(box) or tuple(box.shape) != (nrep, 3, 3):
             raise RuntimeError("box must be a (nreplicas, 3, 3) tensor")
+        if box.dtype != pos.dtype:
+            raise RuntimeError(f"box is {box.dtype} but the positions are {pos.dtype}: one precision per call")
         ctx = self._ensure_ctx(pos)
         self._ensure_box(box)
         L = _lib.lib()
@@ -271,7 +292,8 @@ class Forces:
         stream = torch.cuda.current_stream(pos.device).cuda_stream
         ene = torch.empty((nrep, NUM_ENERGIES), dtype=torch.float64, device=pos.device)
         for _attempt in range(4):
-            _lib.check(L.tmd_forces(ctx, pos.data_ptr(), forces.data_ptr(), ene.data_ptr(), stream))
+            fn = L.tmd_forces_f64 if pos.dtype == torch.float64 else L.tmd_forces
+            _lib.check(fn(ctx, pos.data_ptr(), forces.data_ptr(), ene.data_ptr(), stream))
             if not sync:
                 break
             try:
@@ -332,7 +354,8 @@ class Forces:
 
         pos_in = pos.detach() if torch.is_tensor(pos) and pos.requires_grad else pos
         if forces is None:
-            if self._scratch_forces is None or self._scratch_forces.shape != pos_in.shape:
+            sf = self._scratch_forces
+            if sf is None or sf.shape != pos_in.shape or sf.dtype != pos_in.dtype or sf.device != pos_in.device:
                 self._scratch_forces = torch.empty_like(pos_in)
             forces = self._scratch_forces
         ene = self._evaluate(pos_in, box, forces, exact_gradient=calculateForces and not explicit_forces)
@@ -416,7 +439,8 @@ class Forces:
         count = torch.zeros(1, dtype=torch.int64, device=pos.device)
         cap = max(1024, int(self.stats()["max_neighbours"]) * self.natoms // 2 + 1024)
         out = torch.empty((cap, 2), dtype=torch.int32, device=pos.device)
-        _lib.check(L.tmd_export_pairs(self._ctx, pos.data_ptr(), int(replica), out.data_ptr(), cap, count.data_ptr(), stream))
+        fn = L.tmd_export_pairs_f64 if pos.dtype == torch.float64 else L.tmd_export_pairs
+        _lib.check(fn(self._ctx, pos.data_ptr(), int(replica), out.data_ptr(), cap, count.data_ptr(), stream))
         n = int(count.item())
         if n > cap:
             raise RuntimeError("pair export buffer too small")

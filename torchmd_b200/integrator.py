@@ -77,6 +77,7 @@ class Integrator:
         self.seed = int(torch.randint(0, 2**62, (1,)).item())
         self._step_index = 0
         self._own_ctx = None
+        self._own_dtype = None  # precision the private context was set up for
         self._out = None  # (ke, energies) device buffers, kept between calls: the captured steps hold their addresses
 
     def __del__(self):
@@ -87,18 +88,22 @@ class Integrator:
             pass
 
     def _require_cuda(self):
+        """The state's dtype is the run's precision (float32 or float64); masses and vcoeff follow it."""
         s = self.systems
+        dtype = s.pos.dtype
         for name in ("pos", "vel", "forces"):
             t = getattr(s, name)
             if not _lib.on_device(t):
                 raise RuntimeError(f"systems.{name} must live on a CUDA device: torchmd_b200 has no CPU path")
-            if t.dtype != torch.float32 or not t.is_contiguous():
-                raise NotImplementedError(f"systems.{name} must be contiguous float32")
+            if t.dtype not in (torch.float32, torch.float64) or not t.is_contiguous():
+                raise NotImplementedError(f"systems.{name} must be contiguous float32 or float64")
+            if t.dtype != dtype:
+                raise RuntimeError(f"systems.{name} is {t.dtype} but systems.pos is {dtype}: one precision per run")
         m = self.masses
-        if not _lib.on_device(m) or m.dtype != torch.float32 or not m.is_contiguous():
-            self.masses = m.to(device=s.pos.device, dtype=torch.float32).contiguous()
-        if self.T and (not _lib.on_device(self.vcoeff) or self.vcoeff.dtype != torch.float32 or not self.vcoeff.is_contiguous()):
-            self.vcoeff = self.vcoeff.to(device=s.pos.device, dtype=torch.float32).contiguous()
+        if not _lib.on_device(m) or m.dtype != dtype or not m.is_contiguous():
+            self.masses = m.to(device=s.pos.device, dtype=dtype).contiguous()
+        if self.T and (not _lib.on_device(self.vcoeff) or self.vcoeff.dtype != dtype or not self.vcoeff.is_contiguous()):
+            self.vcoeff = self.vcoeff.to(device=s.pos.device, dtype=dtype).contiguous()
 
     def _ctx(self):
         """Context for the integrator kernels: the Forces object's, or a private one."""
@@ -110,6 +115,15 @@ class Integrator:
             dev = s.pos.device.index if s.pos.device.index is not None else torch.cuda.current_device()
             _lib.check(_lib.lib().tmd_create(C.byref(handle), dev, s.pos.shape[1], s.pos.shape[0]))
             self._own_ctx = handle
+            self._own_dtype = None
+        if self._own_dtype != s.pos.dtype:
+            if self._own_dtype is not None:  # the precision is fixed at set-up: a new context
+                _lib.lib().tmd_destroy(self._own_ctx)
+                self._own_ctx = None
+                return self._ctx()
+            if s.pos.dtype == torch.float64:
+                _lib.check(_lib.lib().tmd_set_precision(self._own_ctx, 64))
+            self._own_dtype = s.pos.dtype
         return self._own_ctx
 
     def step(self, niter=1, noise=None):
@@ -121,13 +135,15 @@ class Integrator:
         ctx = self._ctx()
         stream = torch.cuda.current_stream(s.pos.device).cuda_stream
         nrep = s.pos.shape[0]
+        f64 = s.pos.dtype == torch.float64
+        sfx = "_f64" if f64 else ""
         thermostat = bool(self.T)
         gamma = float(self.gamma) if thermostat else -1.0
         vcoeff = self.vcoeff.data_ptr() if thermostat else None
         if noise is not None:
             if tuple(noise.shape) != (niter,) + tuple(s.vel.shape):
                 raise RuntimeError("noise must have shape (niter, nreplicas, natoms, 3)")
-            noise = noise.to(device=s.pos.device, dtype=torch.float32).contiguous()
+            noise = noise.to(device=s.pos.device, dtype=s.pos.dtype).contiguous()
         if self._out is None or self._out[0].shape[0] != nrep or self._out[0].device != s.pos.device:
             self._out = (torch.empty(nrep, dtype=torch.float64, device=s.pos.device),
                          torch.empty((nrep, _lib.NUM_ENERGIES), dtype=torch.float64, device=s.pos.device))
@@ -147,7 +163,7 @@ class Integrator:
             saved = (s.pos.clone(), s.vel.clone(), s.forces.clone())
             for attempt in range(6):
                 _lib.check(
-                    L.tmd_md_steps(
+                    getattr(L, "tmd_md_steps" + sfx)(
                         ctx, niter, s.pos.data_ptr(), s.vel.data_ptr(), s.forces.data_ptr(), self.masses.data_ptr(),
                         self.dt, gamma, vcoeff, _lib.ptr(noise), self.seed, 0,
                         ene.data_ptr(), ke.data_ptr(), stream,
@@ -170,12 +186,12 @@ class Integrator:
         else:
             for it in range(niter):
                 _lib.check(
-                    L.tmd_vv_first(ctx, s.pos.data_ptr(), s.vel.data_ptr(), s.forces.data_ptr(), self.masses.data_ptr(), self.dt, stream)
+                    getattr(L, "tmd_vv_first" + sfx)(ctx, s.pos.data_ptr(), s.vel.data_ptr(), s.forces.data_ptr(), self.masses.data_ptr(), self.dt, stream)
                 )
                 pot = self.forces.compute(s.pos, s.box, s.forces)
                 last = it == niter - 1
                 _lib.check(
-                    L.tmd_vv_second(
+                    getattr(L, "tmd_vv_second" + sfx)(
                         ctx, s.vel.data_ptr(), s.forces.data_ptr(), self.masses.data_ptr(), self.dt, gamma, vcoeff,
                         noise[it].data_ptr() if noise is not None else None, self.seed, 0,
                         ke.data_ptr() if last else None, stream,
@@ -183,10 +199,10 @@ class Integrator:
                 )
                 self._step_index += 1
             if niter <= 0:
-                _lib.check(L.tmd_kinetic_energy(ctx, s.vel.data_ptr(), self.masses.data_ptr(), ke.data_ptr(), stream))
+                _lib.check(getattr(L, "tmd_kinetic_energy" + sfx)(ctx, s.vel.data_ptr(), self.masses.data_ptr(), ke.data_ptr(), stream))
 
         if self.batch is None:
-            Ekin = ke.cpu().numpy().astype(np.float32)
+            Ekin = ke.cpu().numpy().astype(np.float64 if f64 else np.float32)  # the state's dtype, like integrator.py:122-125
         else:
             Ekin = kinetic_energy(self.masses, s.vel, self.batch).flatten().cpu().numpy()
         T = kinetic_to_temp(Ekin, self.natoms)

@@ -78,17 +78,22 @@ class FrameSink:
     pinned host memory on a side stream and returns; a writer thread appends the frames to
     ``<prefix>_<replica><ext>`` once the copy has completed.  ``save_every``: rewrite the headers
     (make the files loadable) every that many snapshots, like the reference's save period.
+    ``dtype``: of the staging buffers and the files -- torch.float64 for a "precision: double" run
+    (the positions' dtype); the default keeps fp32 files.
     """
 
-    def __init__(self, prefix, ext, natoms, nreplicas, device, save_every=1, nbuffers=2):
+    def __init__(self, prefix, ext, natoms, nreplicas, device, save_every=1, nbuffers=2, dtype=torch.float32):
         self.natoms, self.nrep = int(natoms), int(nreplicas)
         self.device = torch.device(device)
         self.cuda = self.device.type == "cuda"
-        self.files = [NpyAppender(f"{prefix}_{k}{ext}", natoms) for k in range(self.nrep)]
+        if dtype not in (torch.float32, torch.float64):
+            raise ValueError(f"FrameSink writes float32 or float64 frames, not {dtype}")
+        self.files = [NpyAppender(f"{prefix}_{k}{ext}", natoms, dtype=np.float64 if dtype == torch.float64 else np.float32)
+                      for k in range(self.nrep)]
         self.save_every = max(1, int(save_every))
         self._count = 0
-        self._stage = [torch.empty((self.nrep, 3, self.natoms), dtype=torch.float32, device=self.device) for _ in range(nbuffers)]
-        self._host = [torch.empty((self.nrep, 3, self.natoms), dtype=torch.float32, pin_memory=self.cuda) for _ in range(nbuffers)]
+        self._stage = [torch.empty((self.nrep, 3, self.natoms), dtype=dtype, device=self.device) for _ in range(nbuffers)]
+        self._host = [torch.empty((self.nrep, 3, self.natoms), dtype=dtype, pin_memory=self.cuda) for _ in range(nbuffers)]
         self._free = queue.Queue()
         for b in range(nbuffers):
             self._free.put(b)

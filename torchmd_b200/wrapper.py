@@ -4,7 +4,7 @@ Same constructor and ``wrap(pos, box, wrapidx=None)`` call as the reference
 (wrapper.py:4-30; used by run.py:242,266 every output period).  The reference loops over
 the molecule groups in Python -- 33,333 iterations of ~5 torch ops for the 100k-atom water
 box; here the groups are a CSR and one CUDA kernel (csrc/wrap.cuh) moves every group of
-every replica, one warp per group.  CUDA fp32 tensors only, no fallback.
+every replica, one warp per group.  CUDA fp32 or fp64 tensors, no fallback.
 """
 import ctypes as C
 
@@ -93,8 +93,8 @@ class Wrapper:
             # wrapper.py:17-21 rebinds the local name `pos` to a new tensor: everything after it
             # acts on that temporary and the caller's tensor is left untouched.  Same here.
             return
-        if pos.dtype != torch.float32 or box.dtype != torch.float32:
-            raise RuntimeError("torchmd_b200.Wrapper needs fp32 positions and box ('precision: single')")
+        if pos.dtype not in (torch.float32, torch.float64) or box.dtype != pos.dtype:
+            raise RuntimeError("torchmd_b200.Wrapper needs positions and box of one dtype, float32 or float64")
         if pos.dim() != 3 or pos.shape[1] != self.natoms or pos.shape[2] != 3 or tuple(box.shape) != (pos.shape[0], 3, 3):
             raise RuntimeError("wrap: pos must be (nreplicas, natoms, 3) and box (nreplicas, 3, 3)")
         if not pos.is_contiguous() or not box.is_contiguous():
@@ -103,7 +103,8 @@ class Wrapper:
         if not _lib.on_device(pos) or not _lib.on_device(box) or pos.device != self._device or box.device != pos.device:
             raise RuntimeError(f"wrap: pos and box must both live on {self._device} (got {pos.device} and {box.device})")
         stream = torch.cuda.current_stream(pos.device).cuda_stream
-        _lib.check(_lib.lib().tmd_wrapper_wrap(h, pos.data_ptr(), box.data_ptr(), pos.shape[0], stream))
+        fn = _lib.lib().tmd_wrapper_wrap_f64 if pos.dtype == torch.float64 else _lib.lib().tmd_wrapper_wrap
+        _lib.check(fn(h, pos.data_ptr(), box.data_ptr(), pos.shape[0], stream))
 
     def __del__(self):
         h, self._handle = getattr(self, "_handle", None), None
