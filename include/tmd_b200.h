@@ -266,6 +266,32 @@ int tmd_export_pairs_f64(tmd_ctx* ctx, const double* pos_dev, int replica, int32
 int tmd_wrapper_wrap_f64(tmd_wrapper* w, double* pos_dev, const double* box_dev, int nreplicas,
                          tmd_stream stream);
 
+/* ---- constraints: rigid water and bonds to hydrogen (library version >= 102) ----
+ *
+ * tmd_set_constraints holds the constraint tables in the context (host arrays, copied):
+ *   water_idx[3*nwater]   heavy atom, hydrogen, hydrogen of each water
+ *   water_d[2*nwater]     O-H and H-H distance (A)
+ *   cluster_ptr[ncluster+1], cluster_idx: CSR of the X-H clusters, heavy atom first, then its 1-4 hydrogens
+ *   cluster_d             one distance per hydrogen, in cluster_idx order with the heavy atoms left out
+ * No atom may be in two groups.  nwater = ncluster = 0 clears the tables.  The call invalidates the
+ * captured steps of tmd_md_steps.  While tables are set, tmd_md_steps[_f64], tmd_vv_first[_f64] and
+ * tmd_vv_second[_f64] run RATTLE: analytic SETTLE for the waters and SHAKE for the clusters, against
+ * the pre-drift positions after the drift (velocities
+ * corrected by the displacement over dt), the velocity projection after the second half-kick, and
+ * the kinetic energy after it.  tmd_vv_second[_f64] constrains against the positions of the last
+ * tmd_vv_first[_f64] call.  Constraint arithmetic is fp64 in both precisions.  tmd_set_owned_atoms
+ * and tmd_dd_* return TMD_ERR_UNSUPPORTED on a context with constraints.  A water without a SETTLE
+ * solution or a cluster whose SHAKE iteration did not converge is reported by tmd_get_stats
+ * (TMD_ERR_STATE, after its list-overflow report). */
+int tmd_set_constraints(tmd_ctx* ctx, int nwater, const int32_t* water_idx_host, const double* water_d_host,
+                        int ncluster, const int32_t* cluster_ptr_host, const int32_t* cluster_idx_host,
+                        const double* cluster_d_host);
+/* Projects a state onto the constraints: SETTLE / SHAKE with the state's own bond directions, then
+ * (vel_dev not NULL) the velocity projection.  No-op without tables.  Unlike tmd_set_constraints it
+ * takes the masses: a context holds none (the per-step calls pass them, and so does this one). */
+int tmd_constrain(tmd_ctx* ctx, float* pos_dev, float* vel_dev, const float* masses_dev, tmd_stream stream);
+int tmd_constrain_f64(tmd_ctx* ctx, double* pos_dev, double* vel_dev, const double* masses_dev, tmd_stream stream);
+
 /* ---- inspection ------------------------------------------------------------ */
 
 /* The reference's neighbour list for one replica: every non-excluded pair

@@ -10,6 +10,7 @@ from .systems import System  # noqa: F401
 from .forces import Forces  # noqa: F401
 from .integrator import Integrator, kinetic_energy, kinetic_to_temp, maxwell_boltzmann  # noqa: F401
 from .parameters import TopologyParameters  # noqa: F401
+from .constraints import Constraints  # noqa: F401
 from .wrapper import Wrapper  # noqa: F401
 
 __version__ = "0.1.0"

@@ -101,6 +101,10 @@ _SIGNATURES = {
     "tmd_md_steps_f64": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_double, C.c_double, _P, _P, C.c_uint64, C.c_uint64, _P, _P, _P]),
     "tmd_export_pairs_f64": (C.c_int, [_P, _P, C.c_int, _P, C.c_int64, _P, _P]),
     "tmd_wrapper_wrap_f64": (C.c_int, [_P, _P, _P, C.c_int, _P]),
+    # constraints (library version >= 102)
+    "tmd_set_constraints": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, _P, _P, _P]),
+    "tmd_constrain": (C.c_int, [_P, _P, _P, _P, _P]),
+    "tmd_constrain_f64": (C.c_int, [_P, _P, _P, _P, _P]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 
@@ -118,6 +122,8 @@ def lib():
                 "torchmd_b200 has no CPU or PyTorch fallback."
             )
         handle = C.CDLL(LIB_PATH)
+        if not hasattr(handle, "tmd_set_constraints"):
+            raise ImportError(f"{LIB_PATH} predates the constraint entry points: rebuild it (__graft_entry__.build())")
         for name, (res, args) in _SIGNATURES.items():
             fn = getattr(handle, name)
             fn.restype = res

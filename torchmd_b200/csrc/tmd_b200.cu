@@ -22,6 +22,7 @@
 #include "cluster.cuh"
 #include "fused.cuh"
 #include "double.cuh"
+#include "constrain.cuh"
 
 using namespace tmd;
 
@@ -202,6 +203,14 @@ struct CtxPriv {
   std::vector<cudaEvent_t> ev;  // pair-kernel timing samples (begin,end interleaved)
   int ev_used = 0;
   bool profiling = false;
+  // tmd_set_constraints: rigid waters and X-H clusters (constrain.cuh); con_ngroups == 0 means none
+  int con_ngroups = 0, con_nfree = 0;
+  CGroup* con_groups = nullptr;
+  int* con_free = nullptr;
+  double* con_L = nullptr;   // (R,3) box lengths, 0 without a box
+  void* con_ref = nullptr;   // (R,N,3) positions before the drift, in the context's precision
+  int* con_fail = nullptr;   // a group's SHAKE iteration did not converge (tmd_get_stats reports it)
+  const void* con_pos = nullptr;  // positions of the last tmd_vv_first[_f64]: what tmd_vv_second[_f64] constrains against
 };
 
 }  // namespace
@@ -244,7 +253,7 @@ const char* tmd_last_error(void) { return g_err.c_str(); }
 #if defined(TMD_SIMT_HOST)
 int tmd_version(void) { return -100; }  // host SIMT interpreter build (tests/simt): torchmd_b200/_lib.py refuses it
 #else
-int tmd_version(void) { return 101; }  // 101: the "precision: double" entry points (tmd_set_precision, *_f64)
+int tmd_version(void) { return 102; }  // 101: the "precision: double" entry points (tmd_set_precision, *_f64); 102: constraints
 #endif
 
 int tmd_create(tmd_ctx** out, int device, int natoms, int nreplicas) {
@@ -327,6 +336,8 @@ int tmd_destroy(tmd_ctx* ctx) {
   if (priv(ctx).ev_fork) cudaEventDestroy(priv(ctx).ev_fork);
   if (priv(ctx).ev_join) cudaEventDestroy(priv(ctx).ev_join);
   if (priv(ctx).bonded_scratch) cudaFree(priv(ctx).bonded_scratch);
+  for (void* b : {(void*)priv(ctx).con_groups, (void*)priv(ctx).con_free, (void*)priv(ctx).con_L, priv(ctx).con_ref, (void*)priv(ctx).con_fail})
+    if (b) cudaFree(b);
   delete static_cast<tmd_ctx_full*>(ctx);
   return TMD_OK;
 }
@@ -559,6 +570,7 @@ static int set_box(tmd_ctx* ctx, const T* box_diag) {
   ctx->periodic = (nzero == 0);
   ctx->box_host.assign(box_diag, box_diag + ctx->nrep * 3);
   ctx->box64_host.assign(box_diag, box_diag + ctx->nrep * 3);
+  if (priv(ctx).con_L) TMD_CUDA(cudaMemcpy(priv(ctx).con_L, ctx->box64_host.data(), ctx->nrep * 3 * sizeof(double), cudaMemcpyHostToDevice));
   ctx->have_box = true;
   ctx->touched = true;
   priv(ctx).dirty = true;
@@ -1313,6 +1325,67 @@ struct BoundaryArgs {
   uint64_t seed, step;
 };
 
+// ---- constraints (constrain.cuh) ------------------------------------------------------------
+static inline bool has_constraints(tmd_ctx* ctx) { return priv(ctx).con_ngroups > 0; }
+static inline ConstraintTables con_tables(tmd_ctx* ctx) {
+  const CtxPriv& p = priv(ctx);
+  return ConstraintTables{p.con_ngroups, p.con_groups, p.con_nfree, p.con_free, p.con_L};
+}
+// the positions before the drift: the bond directions SHAKE moves the atoms along
+template <typename T>
+static int con_save_ref(tmd_ctx* ctx, const T* pos, cudaStream_t st) {
+  TMD_CUDA(cudaMemcpyAsync(priv(ctx).con_ref, pos, (size_t)ctx->nrep * ctx->natoms * 3 * sizeof(T), cudaMemcpyDeviceToDevice, st));
+  return TMD_OK;
+}
+// ref == nullptr: the positions themselves give the directions (projection of a state)
+template <typename T>
+static int enqueue_constrain_pos(tmd_ctx* ctx, T* pos, const T* ref, T* vel, const T* masses, double dt, cudaStream_t st) {
+  const dim3 g((priv(ctx).con_ngroups + CON_THREADS - 1) / CON_THREADS, ctx->nrep);
+  launch(k_constrain_pos<T, false>, g, CON_THREADS, st, ctx->natoms, con_tables(ctx), pos, ref ? ref : pos, vel, masses,
+         dt > 0.0 ? 1.0 / dt : 0.0, priv(ctx).con_fail, ctx->d);
+  TMD_LAUNCHED(ctx, "k_constrain_pos");
+  return TMD_OK;
+}
+// tmd_md_steps (fp32, whole system, TMD_B200_FUSEPREP): the position constraint also prepares the force call that
+// follows on this stream (list check, slot records), as k_vv_first_prepare does without constraints
+static bool con_can_prepare(tmd_ctx* ctx) { return priv(ctx).fuse_prepare && ctx->d.own_all && ctx->pair_mask; }
+static int enqueue_constrain_pos_prepare(tmd_ctx* ctx, float* pos, const float* ref, float* vel, const float* masses, double dt,
+                                         cudaStream_t st) {
+  CtxPriv& pv = priv(ctx);
+  DeviceState dp = ctx->d;
+  pv.prepared_cond = 0;
+  if (pv.use_cond) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    cudaGraph_t cap_graph = nullptr;
+    if (cudaStreamGetCaptureInfo(st, &cs, nullptr, &cap_graph, nullptr, nullptr) == cudaSuccess &&
+        cs == cudaStreamCaptureStatusActive && cap_graph) {
+      TMD_CUDA(cudaGraphConditionalHandleCreate(&pv.prepared_cond, cap_graph, 0, cudaGraphCondAssignDefault));
+      dp.cond = (unsigned long long)pv.prepared_cond;
+    }
+  }
+  const dim3 g((pv.con_ngroups + pv.con_nfree + CON_THREADS - 1) / CON_THREADS, ctx->nrep);
+  launch(k_constrain_pos<float, true>, g, CON_THREADS, st, ctx->natoms, con_tables(ctx), pos, ref, vel, masses, 1.0 / dt,
+         pv.con_fail, dp);
+  TMD_LAUNCHED(ctx, "k_constrain_pos");
+  pv.prepared = true;
+  return TMD_OK;
+}
+// velocity projection; with ke, the kinetic energy after it
+template <typename T>
+static int enqueue_constrain_vel(tmd_ctx* ctx, const T* pos, T* vel, const T* masses, double* ke, cudaStream_t st) {
+  const CtxPriv& p = priv(ctx);
+  const int items = p.con_ngroups + (ke ? p.con_nfree : 0);
+  const dim3 g((items + CON_THREADS - 1) / CON_THREADS, ctx->nrep);
+  if (ke) {
+    TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
+    launch(k_constrain_vel<T, true>, g, CON_THREADS, st, ctx->natoms, con_tables(ctx), pos, vel, masses, ke);
+  } else {
+    launch(k_constrain_vel<T, false>, g, CON_THREADS, st, ctx->natoms, con_tables(ctx), pos, vel, masses, ke);
+  }
+  TMD_LAUNCHED(ctx, "k_constrain_vel");
+  return TMD_OK;
+}
+
 static int enqueue_vv_first(tmd_ctx* ctx, float* pos, float* vel, const float* forces, const float* masses,
                             double dt, cudaStream_t st, bool forces_follow = false, const BoundaryArgs* boundary = nullptr) {
   CtxPriv& pv = priv(ctx);
@@ -1430,7 +1503,12 @@ int tmd_vv_first(tmd_ctx* ctx, float* pos, float* vel, const float* forces, cons
   if (!ctx || !pos || !vel || !forces || !masses) return fail(TMD_ERR_ARG, "tmd_vv_first: null pointer");
   TMD_PRECISION(ctx, 32, "tmd_vv_first")
   DeviceGuard guard(ctx->device);
-  return enqueue_vv_first(ctx, pos, vel, forces, masses, dt, (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (!has_constraints(ctx)) return enqueue_vv_first(ctx, pos, vel, forces, masses, dt, st);
+  int rc;
+  if ((rc = con_save_ref(ctx, pos, st)) || (rc = enqueue_vv_first(ctx, pos, vel, forces, masses, dt, st))) return rc;
+  priv(ctx).con_pos = pos;
+  return enqueue_constrain_pos(ctx, pos, static_cast<const float*>(priv(ctx).con_ref), vel, masses, dt, st);
 }
 
 int tmd_vv_second(tmd_ctx* ctx, float* vel, const float* forces, const float* masses, double dt, double gamma,
@@ -1439,8 +1517,12 @@ int tmd_vv_second(tmd_ctx* ctx, float* vel, const float* forces, const float* ma
   if (!ctx || !vel || !forces || !masses) return fail(TMD_ERR_ARG, "tmd_vv_second: null pointer");
   TMD_PRECISION(ctx, 32, "tmd_vv_second")
   DeviceGuard guard(ctx->device);
-  return enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step_index, ke,
-                           (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (!has_constraints(ctx)) return enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step_index, ke, st);
+  if (!priv(ctx).con_pos) return fail(TMD_ERR_STATE, "tmd_vv_second: constraints are set but tmd_vv_first has not run");
+  int rc;
+  if ((rc = enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step_index, nullptr, st))) return rc;
+  return enqueue_constrain_vel(ctx, static_cast<const float*>(priv(ctx).con_pos), vel, masses, ke, st);
 }
 
 int tmd_kinetic_energy(tmd_ctx* ctx, const float* vel, const float* masses, double* ke, tmd_stream stream) {
@@ -1480,8 +1562,13 @@ int tmd_md_steps(tmd_ctx* ctx, int niter, float* pos, float* vel, float* forces,
   } fold_scope(pv, pv.fuse_prepare);
   // TMD_B200_FUSESTEP: inside one call the second half of a step and the first half of the next are one kernel
   // (cluster path with the bonded kernel on the side stream: the force call leaves its fold to the integrator)
+  // With constraints the step is RATTLE: the position constraint sits between the drift and the force call and the
+  // velocity constraint after the second half-kick, so neither the boundary kernel nor the fused prepare applies.
+  const bool con = has_constraints(ctx);
   const bool fuse = pv.fuse_step && pv.fuse_prepare && ctx->d.cl.on && ctx->d.own_all && ctx->pair_mask && !noise &&
-                    ctx->bonded_nentries > 0 && pv.side != nullptr && niter >= 2;
+                    ctx->bonded_nentries > 0 && pv.side != nullptr && niter >= 2 && !con;
+  const float* cref = static_cast<const float*>(pv.con_ref);
+  if (con) pv.con_pos = pos;
   const BoundaryArgs bargs{gamma, vcoeff, seed, first_step};
   if (pv.use_graph && !noise && !pv.profiling && niter > 0) {
     // One MD step captured once (with and without the energy outputs) and replayed: one graph
@@ -1508,10 +1595,15 @@ int tmd_md_steps(tmd_ctx* ctx, int niter, float* pos, float* vel, float* forces,
         const bool with_e = (k == 1 || k == 4), opens_with_boundary = (k >= 3), closes = (k != 2 && k != 3);
         const int64_t l0 = ctx->launches, f0 = ctx->force_calls;
         TMD_CUDA(cudaStreamBeginCapture(pv.gstream, cudaStreamCaptureModeRelaxed));
-        int rc2 = enqueue_vv_first(ctx, pos, vel, forces, masses, dt, pv.gstream, true, opens_with_boundary ? &bargs : nullptr);
+        int rc2 = con ? con_save_ref(ctx, pos, pv.gstream) : TMD_OK;
+        if (!rc2) rc2 = enqueue_vv_first(ctx, pos, vel, forces, masses, dt, pv.gstream, !con, opens_with_boundary ? &bargs : nullptr);
+        if (!rc2 && con)
+          rc2 = con_can_prepare(ctx) ? enqueue_constrain_pos_prepare(ctx, pos, cref, vel, masses, dt, pv.gstream)
+                                     : enqueue_constrain_pos(ctx, pos, cref, vel, masses, dt, pv.gstream);
         if (!rc2) rc2 = enqueue_forces(ctx, pos, forces, with_e ? energies : nullptr, pv.gstream);
         if (!rc2 && closes) rc2 = enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, nullptr, seed, first_step,
-                                                    with_e ? ke : nullptr, pv.gstream);
+                                                    with_e && !con ? ke : nullptr, pv.gstream);
+        if (!rc2 && closes && con) rc2 = enqueue_constrain_vel(ctx, pos, vel, masses, with_e ? ke : nullptr, pv.gstream);
         pv.fold_pending = false;  // (variants 2 and 3 leave the fold to the graph that follows)
         cudaError_t ce = cudaStreamEndCapture(pv.gstream, &pv.graph[k]);
         if (rc2) return rc2;
@@ -1550,12 +1642,17 @@ int tmd_md_steps(tmd_ctx* ctx, int niter, float* pos, float* vel, float* forces,
   }
   for (int it = 0; it < niter; ++it) {
     const bool last = (it == niter - 1);
-    if ((rc = enqueue_vv_first(ctx, pos, vel, forces, masses, dt, st, true, fuse && it > 0 ? &bargs : nullptr))) return rc;
+    if (con && (rc = con_save_ref(ctx, pos, st))) return rc;
+    if ((rc = enqueue_vv_first(ctx, pos, vel, forces, masses, dt, st, !con, fuse && it > 0 ? &bargs : nullptr))) return rc;
+    if (con && (rc = con_can_prepare(ctx) ? enqueue_constrain_pos_prepare(ctx, pos, cref, vel, masses, dt, st)
+                                          : enqueue_constrain_pos(ctx, pos, cref, vel, masses, dt, st)))
+      return rc;
     if ((rc = enqueue_forces(ctx, pos, forces, last ? energies : nullptr, st))) return rc;
     if (fuse && !last) continue;  // the next iteration's boundary kernel finishes this step
     if ((rc = enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise ? noise + it * per_step : nullptr,
-                                seed, first_step, last ? ke : nullptr, st)))
+                                seed, first_step, last && !con ? ke : nullptr, st)))
       return rc;
+    if (con && (rc = enqueue_constrain_vel(ctx, pos, vel, masses, last ? ke : nullptr, st))) return rc;
   }
   return TMD_OK;
 }
@@ -1622,9 +1719,15 @@ int tmd_vv_first_f64(tmd_ctx* ctx, double* pos, double* vel, const double* force
   if (!ctx || !pos || !vel || !forces || !masses) return fail(TMD_ERR_ARG, "tmd_vv_first_f64: null pointer");
   TMD_PRECISION(ctx, 64, "tmd_vv_first_f64")
   DeviceGuard guard(ctx->device);
-  enqueue_vv_first_f64(ctx, pos, vel, forces, masses, dt, (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool con = has_constraints(ctx);
+  int rc;
+  if (con && (rc = con_save_ref(ctx, pos, st))) return rc;
+  enqueue_vv_first_f64(ctx, pos, vel, forces, masses, dt, st);
   TMD_LAUNCHED(ctx, "k_vv_first_f64");
-  return TMD_OK;
+  if (!con) return TMD_OK;
+  priv(ctx).con_pos = pos;
+  return enqueue_constrain_pos(ctx, pos, static_cast<const double*>(priv(ctx).con_ref), vel, masses, dt, st);
 }
 
 int tmd_vv_second_f64(tmd_ctx* ctx, double* vel, const double* forces, const double* masses, double dt, double gamma,
@@ -1634,9 +1737,12 @@ int tmd_vv_second_f64(tmd_ctx* ctx, double* vel, const double* forces, const dou
   TMD_PRECISION(ctx, 64, "tmd_vv_second_f64")
   DeviceGuard guard(ctx->device);
   cudaStream_t st = (cudaStream_t)stream;
-  if (ke) TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
-  enqueue_vv_second_f64(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step_index, ke, st);
+  const bool con = has_constraints(ctx);
+  if (con && !priv(ctx).con_pos) return fail(TMD_ERR_STATE, "tmd_vv_second_f64: constraints are set but tmd_vv_first_f64 has not run");
+  if (ke && !con) TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
+  enqueue_vv_second_f64(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step_index, con ? nullptr : ke, st);
   TMD_LAUNCHED(ctx, "k_vv_second_f64");
+  if (con) return enqueue_constrain_vel(ctx, static_cast<const double*>(priv(ctx).con_pos), vel, masses, ke, st);
   return TMD_OK;
 }
 
@@ -1661,15 +1767,22 @@ int tmd_md_steps_f64(tmd_ctx* ctx, int niter, double* pos, double* vel, double* 
   int rc;
   if (priv(ctx).dirty && (rc = finalize(ctx, st))) return rc;
   const size_t per_step = (size_t)ctx->nrep * ctx->natoms * 3;
+  const bool con = has_constraints(ctx);  // RATTLE: see tmd_md_steps
+  const double* cref = static_cast<const double*>(priv(ctx).con_ref);
+  if (con) priv(ctx).con_pos = pos;
   for (int it = 0; it < niter; ++it) {
     const bool last = (it == niter - 1);
+    if (con && (rc = con_save_ref(ctx, pos, st))) return rc;
     enqueue_vv_first_f64(ctx, pos, vel, forces, masses, dt, st);
     TMD_LAUNCHED(ctx, "k_vv_first_f64");
+    if (con && (rc = enqueue_constrain_pos(ctx, pos, cref, vel, masses, dt, st))) return rc;
     if ((rc = enqueue_forces_f64(ctx, pos, forces, last ? energies : nullptr, st))) return rc;
-    if (last && ke) TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
+    double* ke2 = last && !con ? ke : nullptr;
+    if (ke2) TMD_CUDA(cudaMemsetAsync(ke2, 0, (size_t)ctx->nrep * sizeof(double), st));
     enqueue_vv_second_f64(ctx, vel, forces, masses, dt, gamma, vcoeff, noise ? noise + it * per_step : nullptr, seed, first_step,
-                          last ? ke : nullptr, st);
+                          ke2, st);
     TMD_LAUNCHED(ctx, "k_vv_second_f64");
+    if (con && (rc = enqueue_constrain_vel(ctx, pos, vel, masses, last ? ke : nullptr, st))) return rc;
   }
   return TMD_OK;
 }
@@ -1729,6 +1842,7 @@ int tmd_set_owned_atoms(tmd_ctx* ctx, int first_atom, int count) {
   if (!ctx || first_atom < 0 || count < 0 || first_atom + count > ctx->natoms)
     return fail(TMD_ERR_ARG, "tmd_set_owned_atoms: range outside the system");
   if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_owned_atoms: fp64 contexts run the whole system on one GPU");
+  if (has_constraints(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_owned_atoms: a context with constraints runs the whole system on one GPU");
   ctx->d.own_lo = first_atom;
   ctx->d.own_n = count;
   ctx->d.own_all = (first_atom == 0 && count == ctx->natoms) ? 1 : 0;
@@ -1736,11 +1850,106 @@ int tmd_set_owned_atoms(tmd_ctx* ctx, int first_atom, int count) {
   return TMD_OK;
 }
 
+// ---- constraints ---------------------------------------------------------------------------
+int tmd_set_constraints(tmd_ctx* ctx, int nwater, const int32_t* water_idx, const double* water_d, int ncluster,
+                        const int32_t* cluster_ptr, const int32_t* cluster_idx, const double* cluster_d) {
+  if (!ctx || nwater < 0 || ncluster < 0 || (nwater && (!water_idx || !water_d)) ||
+      (ncluster && (!cluster_ptr || !cluster_idx || !cluster_d)))
+    return fail(TMD_ERR_ARG, "tmd_set_constraints: bad arguments");
+  if (ctx->dd_base || !ctx->d.own_all)
+    return fail(TMD_ERR_UNSUPPORTED, "tmd_set_constraints: decomposed runs cannot hold constraints");
+  const int N = ctx->natoms;
+  std::vector<CGroup> groups;
+  groups.reserve((size_t)nwater + ncluster);
+  std::vector<char> used(N, 0);
+  auto take = [&](int a) { return a >= 0 && a < N && !used[a] ? (used[a] = 1, true) : false; };
+  for (int w = 0; w < nwater; ++w) {
+    CGroup g{};
+    g.na = 3;
+    g.nc = 3;
+    for (int j = 0; j < 3; ++j) g.atom[j] = water_idx[3 * w + j];
+    const int ca[3] = {0, 0, 1}, cb[3] = {1, 2, 2};
+    const double d[3] = {water_d[2 * w], water_d[2 * w], water_d[2 * w + 1]};  // O-H, O-H, H-H
+    for (int c = 0; c < 3; ++c) {
+      g.ca[c] = ca[c];
+      g.cb[c] = cb[c];
+      g.d[c] = d[c];
+      if (!(d[c] > 0.0)) return fail(TMD_ERR_ARG, "tmd_set_constraints: a water distance is not positive");
+    }
+    for (int j = 0; j < 3; ++j)
+      if (!take(g.atom[j])) return fail(TMD_ERR_ARG, "tmd_set_constraints: atom out of range or in two constraint groups");
+    groups.push_back(g);
+  }
+  for (int c = 0; c < ncluster; ++c) {
+    const int lo = cluster_ptr[c], hi = cluster_ptr[c + 1];  // cluster_idx[lo]: heavy atom, then its hydrogens
+    if (lo < 0 || hi - lo < 2 || hi - lo > CON_MAX_ATOMS)
+      return fail(TMD_ERR_ARG, "tmd_set_constraints: a cluster has one heavy atom and 1-4 hydrogens");
+    CGroup g{};
+    g.na = hi - lo;
+    g.nc = g.na - 1;
+    for (int j = 0; j < g.na; ++j) {
+      g.atom[j] = cluster_idx[lo + j];
+      if (!take(g.atom[j])) return fail(TMD_ERR_ARG, "tmd_set_constraints: atom out of range or in two constraint groups");
+    }
+    for (int k = 0; k < g.nc; ++k) {
+      g.ca[k] = 0;
+      g.cb[k] = k + 1;
+      g.d[k] = cluster_d[lo + k - c];  // one distance per hydrogen: cluster_d is indexed like cluster_idx without the heavy atoms
+      if (!(g.d[k] > 0.0)) return fail(TMD_ERR_ARG, "tmd_set_constraints: a cluster distance is not positive");
+    }
+    groups.push_back(g);
+  }
+  std::vector<int> free_atoms;
+  for (int i = 0; i < N; ++i)
+    if (!used[i]) free_atoms.push_back(i);
+  DeviceGuard guard(ctx->device);
+  CtxPriv& p = priv(ctx);
+  p.steps_valid = false;  // the captured steps do not hold the constraint kernels (or hold stale ones)
+  p.con_pos = nullptr;
+  p.con_ngroups = 0;
+  p.con_nfree = 0;
+  if (groups.empty()) return TMD_OK;
+  int rc;
+  if ((rc = upload(&p.con_groups, groups.data(), groups.size()))) return rc;
+  if ((rc = upload(&p.con_free, free_atoms.data(), free_atoms.size()))) return rc;
+  std::vector<double> L = ctx->have_box ? ctx->box64_host : std::vector<double>((size_t)ctx->nrep * 3, 0.0);
+  if ((rc = upload(&p.con_L, L.data(), L.size()))) return rc;
+  if (!p.con_ref && (rc = device_alloc(reinterpret_cast<double**>(&p.con_ref), (size_t)ctx->nrep * N * 3))) return rc;
+  if (!p.con_fail && (rc = device_alloc(&p.con_fail, 1))) return rc;
+  TMD_CUDA(cudaMemset(p.con_fail, 0, sizeof(int)));
+  p.con_ngroups = (int)groups.size();
+  p.con_nfree = (int)free_atoms.size();
+  return TMD_OK;
+}
+
+extern "C++" {  // (templates inside the C-linkage block)
+template <typename T>
+static int constrain_state(tmd_ctx* ctx, T* pos, T* vel, const T* masses, tmd_stream stream, const char* name) {
+  if (!ctx || !pos || !masses) return fail(TMD_ERR_ARG, std::string(name) + ": null pointer");
+  DeviceGuard guard(ctx->device);
+  if (!has_constraints(ctx)) return TMD_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  if ((rc = enqueue_constrain_pos(ctx, pos, (const T*)nullptr, (T*)nullptr, masses, 0.0, st))) return rc;
+  if (vel && (rc = enqueue_constrain_vel(ctx, (const T*)pos, vel, masses, nullptr, st))) return rc;
+  return TMD_OK;
+}
+}  // extern "C++"
+int tmd_constrain(tmd_ctx* ctx, float* pos, float* vel, const float* masses, tmd_stream stream) {
+  if (ctx) TMD_PRECISION(ctx, 32, "tmd_constrain")
+  return constrain_state(ctx, pos, vel, masses, stream, "tmd_constrain");
+}
+int tmd_constrain_f64(tmd_ctx* ctx, double* pos, double* vel, const double* masses, tmd_stream stream) {
+  if (ctx) TMD_PRECISION(ctx, 64, "tmd_constrain_f64")
+  return constrain_state(ctx, pos, vel, masses, stream, "tmd_constrain_f64");
+}
+
 // ---- peer-to-peer position exchange (helpers above, next to priv()) ------------------------
 int tmd_dd_create(tmd_ctx* ctx, int rank, int world, unsigned char* handle_out) {
   if (!ctx || !handle_out || world < 1 || world > TMD_MAX_PEERS || rank < 0 || rank >= world)
     return fail(TMD_ERR_ARG, "tmd_dd_create: bad arguments (at most 16 ranks)");
   if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_create: fp64 contexts run the whole system on one GPU");
+  if (has_constraints(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_create: a context with constraints runs the whole system on one GPU");
   if (ctx->nrep != 1) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_create: decomposed runs take one replica");
   static_assert(sizeof(cudaIpcMemHandle_t) == TMD_IPC_HANDLE_BYTES, "IPC handle size");
   DeviceGuard guard(ctx->device);
@@ -1764,6 +1973,7 @@ int tmd_dd_create(tmd_ctx* ctx, int rank, int world, unsigned char* handle_out) 
 int tmd_dd_connect(tmd_ctx* ctx, const unsigned char* handles) {
   if (!ctx || !handles) return fail(TMD_ERR_ARG, "tmd_dd_connect: null pointer");
   if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_connect: fp64 contexts run the whole system on one GPU");
+  if (has_constraints(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_connect: a context with constraints runs the whole system on one GPU");
   if (!ctx->dd_base) return fail(TMD_ERR_STATE, "tmd_dd_connect: tmd_dd_create has not been called");
   DeviceGuard guard(ctx->device);
   for (int p = 0; p < ctx->dd_world; ++p) {
@@ -1781,6 +1991,7 @@ int tmd_dd_connect(tmd_ctx* ctx, const unsigned char* handles) {
 #define TMD_DD_READY(name)                                                                     \
   if (!ctx) return fail(TMD_ERR_ARG, name ": null context");                                   \
   if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, name ": fp64 contexts run the whole system on one GPU"); \
+  if (has_constraints(ctx)) return fail(TMD_ERR_UNSUPPORTED, name ": a context with constraints runs the whole system on one GPU"); \
   if (!ctx->dd_connected) return fail(TMD_ERR_STATE, name ": tmd_dd_create / tmd_dd_connect first"); \
   DeviceGuard guard(ctx->device);
 
@@ -1943,7 +2154,19 @@ int tmd_get_stats(tmd_ctx* ctx, tmd_stats* out, tmd_stream stream) {
   out->kernel_launches = ctx->launches;
   out->row_capacity = ctx->d.row_cap;
   out->rebuilds = ctx->rebuilds_before;
-  if (priv(ctx).dirty || !ctx->d.flags) return TMD_OK;
+  // a constraint group without a solution since the last check: reported after the list checks below, whose
+  // overflow makes the caller run the steps again (a truncated force can be what broke the constraint)
+  int con_failed = 0;
+  if (priv(ctx).con_fail) {
+    TMD_CUDA(cudaMemcpy(&con_failed, priv(ctx).con_fail, sizeof(int), cudaMemcpyDeviceToHost));
+    if (con_failed) TMD_CUDA(cudaMemset(priv(ctx).con_fail, 0, sizeof(int)));
+  }
+  auto con_error = [&]() {
+    return con_failed ? fail(TMD_ERR_STATE, "a constraint group has no solution (SETTLE) or SHAKE did not converge: the "
+                                            "time step is too long or the system blew up")
+                      : TMD_OK;
+  };
+  if (priv(ctx).dirty || !ctx->d.flags) return con_error();
   std::vector<int> fl((size_t)ctx->nrep * F_COUNT);
   TMD_CUDA(cudaMemcpy(fl.data(), ctx->d.flags, fl.size() * sizeof(int), cudaMemcpyDeviceToHost));
   Grid g0;
@@ -2000,7 +2223,7 @@ int tmd_get_stats(tmd_ctx* ctx, tmd_stats* out, tmd_stream stream) {
       priv(ctx).dirty = true;
       return fail(TMD_ERR_OVERFLOW, "cluster list capacity exceeded; capacity grown, recompute required");
     }
-    return TMD_OK;
+    return con_error();
   }
   if (overflow) {
     // grow the rows, invalidate the list; the caller recomputes (standalone force call)
@@ -2009,7 +2232,7 @@ int tmd_get_stats(tmd_ctx* ctx, tmd_stats* out, tmd_stream stream) {
     priv(ctx).dirty = true;
     return fail(TMD_ERR_OVERFLOW, "neighbour row capacity exceeded; capacity grown, recompute required");
   }
-  return TMD_OK;
+  return con_error();
 }
 
 }  // extern "C"

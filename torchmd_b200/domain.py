@@ -85,7 +85,9 @@ class DecomposedIntegrator:
     construction ``system.pos`` aliases a padded gather buffer.  Single replica only.
     """
 
-    def __init__(self, system, forces, timestep, device, gamma=None, T=None, group=None, use_graph=True, exchange=None):
+    def __init__(self, system, forces, timestep, device, gamma=None, T=None, group=None, use_graph=True, exchange=None, constraints=None):
+        if constraints is not None:
+            raise NotImplementedError("constraints run on one GPU: use Integrator(..., constraints=...)")
         if system.pos.dtype == torch.float64:
             raise NotImplementedError("decomposed runs are fp32 only: run 'precision: double' on one GPU")
         if system.pos.shape[0] != 1:

@@ -8,6 +8,10 @@ whole ``niter`` loop is enqueued through one C-ABI call with no host round trip
 (the reference synchronises several times per step, SURVEY.md section 3.3);
 any other object exposing ``compute(pos, box, forces)`` is driven step by step
 exactly like the reference does (``tests/test_integrator.py`` mock forces).
+
+``constraints`` (a ``torchmd_b200.constraints.Constraints``) makes the step RATTLE: rigid waters and,
+with ``kind="hbonds"``, fixed bonds to hydrogen, which allow 2 fs time steps.  The returned ``T`` then
+counts the constrained degrees of freedom out (``Constraints.ndof``); ``Ekin`` stays sum(m v^2 / 2).
 """
 import ctypes as C
 
@@ -49,7 +53,7 @@ def kinetic_to_temp(Ekin, natoms):
 
 
 class Integrator:
-    def __init__(self, systems, forces, timestep, device, gamma=None, T=None, batch=None):
+    def __init__(self, systems, forces, timestep, device, gamma=None, T=None, batch=None, constraints=None):
         self.dt = timestep / TIMEFACTOR
         self.systems = systems
         self.forces = forces
@@ -79,6 +83,12 @@ class Integrator:
         self._own_ctx = None
         self._own_dtype = None  # precision the private context was set up for
         self._out = None  # (ke, energies) device buffers, kept between calls: the captured steps hold their addresses
+        self.constraints = constraints
+        self._projected = False  # the start state has been projected onto the constraints
+        if constraints is not None:
+            if constraints.natoms != len(self.masses):
+                raise ValueError(f"constraints are for {constraints.natoms} atoms, the system has {len(self.masses)}")
+            self.ndof = constraints.ndof(batch=batch.cpu().numpy() if batch is not None else None)
 
     def __del__(self):
         try:
@@ -126,13 +136,26 @@ class Integrator:
             self._own_dtype = s.pos.dtype
         return self._own_ctx
 
+    def _constrained_ctx(self):
+        """``_ctx()`` holding this integrator's constraint tables, or none.  The tables live in the context, which a
+        ``Forces`` object shares between the integrators built on it: the handle records which ``Constraints`` it
+        holds, and the tables are handed over (or cleared) whenever that is not this integrator's."""
+        ctx = self._ctx()
+        if getattr(ctx, "_tmd_constraints", None) is not self.constraints:
+            if self.constraints is not None:
+                self.constraints.upload(ctx)
+            else:
+                _lib.check(_lib.lib().tmd_set_constraints(ctx, 0, None, None, 0, None, None, None))
+            ctx._tmd_constraints = self.constraints
+        return ctx
+
     def step(self, niter=1, noise=None):
         """Advance ``niter`` steps.  ``noise`` (niter, R, N, 3) injects the N(0,1) Langevin
         draws (parity tests); by default they come from Philox4x32-10 inside the kernel."""
         s = self.systems
         self._require_cuda()
         L = _lib.lib()
-        ctx = self._ctx()
+        ctx = self._constrained_ctx()
         stream = torch.cuda.current_stream(s.pos.device).cuda_stream
         nrep = s.pos.shape[0]
         f64 = s.pos.dtype == torch.float64
@@ -148,6 +171,10 @@ class Integrator:
             self._out = (torch.empty(nrep, dtype=torch.float64, device=s.pos.device),
                          torch.empty((nrep, _lib.NUM_ENERGIES), dtype=torch.float64, device=s.pos.device))
         ke = self._out[0]
+        if self.constraints is not None and not self._projected:
+            # a start state (maxwell_boltzmann velocities above all) has components along the constrained bonds
+            _lib.check(getattr(L, "tmd_constrain" + sfx)(ctx, s.pos.data_ptr(), s.vel.data_ptr(), self.masses.data_ptr(), stream))
+            self._projected = True
         native = isinstance(self.forces, Forces) and not self.forces.external
         pot = None
         if native and niter > 0:
@@ -180,7 +207,7 @@ class Integrator:
                     s.pos.copy_(saved[0])
                     s.vel.copy_(saved[1])
                     s.forces.copy_(saved[2])
-                    ctx = self._ctx()  # (re-finalised with the grown capacity on the next call)
+                    ctx = self._constrained_ctx()  # (re-finalised with the grown capacity on the next call)
             self._step_index += niter
             pot = f._format(ene, None, s.pos.dtype, False, True)
         else:
@@ -200,10 +227,15 @@ class Integrator:
                 self._step_index += 1
             if niter <= 0:
                 _lib.check(getattr(L, "tmd_kinetic_energy" + sfx)(ctx, s.vel.data_ptr(), self.masses.data_ptr(), ke.data_ptr(), stream))
+            elif self.constraints is not None:  # (the fused path learns of a failed constraint group from f.stats())
+                _lib.check(L.tmd_get_stats(ctx, C.byref(_lib.Stats()), stream))
 
         if self.batch is None:
             Ekin = ke.cpu().numpy().astype(np.float64 if f64 else np.float32)  # the state's dtype, like integrator.py:122-125
         else:
             Ekin = kinetic_energy(self.masses, s.vel, self.batch).flatten().cpu().numpy()
-        T = kinetic_to_temp(Ekin, self.natoms)
+        if self.constraints is None:
+            T = kinetic_to_temp(Ekin, self.natoms)
+        else:
+            T = 2.0 / (self.ndof * BOLTZMAN) * Ekin
         return Ekin, pot, T
