@@ -292,6 +292,32 @@ int tmd_set_constraints(tmd_ctx* ctx, int nwater, const int32_t* water_idx_host,
 int tmd_constrain(tmd_ctx* ctx, float* pos_dev, float* vel_dev, const float* masses_dev, tmd_stream stream);
 int tmd_constrain_f64(tmd_ctx* ctx, double* pos_dev, double* vel_dev, const double* masses_dev, tmd_stream stream);
 
+/* ---- particle-mesh Ewald electrostatics (library version >= 103) ----
+ *
+ * tmd_set_pme(ctx, tolerance > 0) turns PME on; tolerance <= 0 turns it off.  Call it after
+ * tmd_set_nonbonded: it needs the electrostatics term, a cutoff and no reaction field
+ * (TMD_ERR_UNSUPPORTED otherwise).  The electrostatic energy slot then holds
+ *   real space    sum k qi qj erfc(alpha r) / r over the cutoff's pair set (no shift, no switch)
+ *   reciprocal    smooth PME, order-5 B-splines, fp64 accumulation
+ *   exclusions    - sum k qi qj erf(alpha r) / r over the excluded pairs (minimum image)
+ *   self          - k alpha / sqrt(pi) sum qi^2
+ *   background    - k pi Q^2 / (2 V alpha^2), Q the net charge
+ * and the forces are its exact gradient.  alpha = sqrt(-ln 2 tol) / cutoff and the grid
+ * n_d = smallest 2^a 3^b 5^c >= max(2 alpha L_d / (3 tol^(1/5)), 10), the largest over the
+ * replicas, are chosen here and again by every tmd_set_box[_f64]; each replica keeps its own box
+ * and influence function.  tmd_set_box[_f64] returns TMD_ERR_UNSUPPORTED for a box that is not
+ * periodic, a cutoff above half a box length on any axis, or a grid above 512 points on an axis.
+ * The reciprocal forces are bitwise reproducible (fixed-point charge grid, per-atom gather).
+ * The exclusion correction reads the rows of tmd_set_exclusions as the set of excluded pairs: each pair
+ * must appear in both atoms' rows, once, and no atom in its own row; otherwise the first force call
+ * returns TMD_ERR_ARG.  The real-space term is cut at the cutoff without a shift, so energy
+ * conservation improves with a smaller tolerance (DESIGN.md §5b).
+ * tmd_set_owned_atoms and tmd_dd_* return TMD_ERR_UNSUPPORTED on a PME context.
+ * tmd_get_pme reports the chosen alpha (1/A) and grid (TMD_ERR_STATE while PME is off or no box
+ * has been set). */
+int tmd_set_pme(tmd_ctx* ctx, double tolerance);
+int tmd_get_pme(tmd_ctx* ctx, double* alpha, int32_t grid[3]);
+
 /* ---- inspection ------------------------------------------------------------ */
 
 /* The reference's neighbour list for one replica: every non-excluded pair
@@ -304,7 +330,8 @@ int tmd_export_pairs(tmd_ctx* ctx, const float* pos_dev, int replica, int32_t* p
 /* Which pair kernel the last tmd_forces / tmd_md_steps launched: 0 k_pair (float separations, the
  * default), 1 k_pair_fx (fixed-point separations), 2 k_pair_fx2 (fixed point + fp32x2
  * arithmetic), 3 k_pair2_open (no box, fp32x2 arithmetic), 4 k_cpair (cluster lists),
- * 5 k_pair_f64 (fp64 context).  For tests and bench labels. */
+ * 5 k_pair_f64 (fp64 context); with particle-mesh Ewald, the real-space Ewald instantiations
+ * 6 k_pair<MODE 2>, 7 k_pair_fx<MODE 2>, 8 k_ewpair64 (fp64).  For tests and bench labels. */
 int tmd_pair_kernel(tmd_ctx* ctx);
 
 typedef struct {

@@ -105,6 +105,9 @@ _SIGNATURES = {
     "tmd_set_constraints": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, _P, _P, _P]),
     "tmd_constrain": (C.c_int, [_P, _P, _P, _P, _P]),
     "tmd_constrain_f64": (C.c_int, [_P, _P, _P, _P, _P]),
+    # particle-mesh Ewald (library version >= 103)
+    "tmd_set_pme": (C.c_int, [_P, C.c_double]),
+    "tmd_get_pme": (C.c_int, [_P, C.POINTER(C.c_double), C.POINTER(C.c_int32 * 3)]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 
@@ -122,8 +125,8 @@ def lib():
                 "torchmd_b200 has no CPU or PyTorch fallback."
             )
         handle = C.CDLL(LIB_PATH)
-        if not hasattr(handle, "tmd_set_constraints"):
-            raise ImportError(f"{LIB_PATH} predates the constraint entry points: rebuild it (__graft_entry__.build())")
+        if not hasattr(handle, "tmd_set_pme"):
+            raise ImportError(f"{LIB_PATH} predates the particle-mesh Ewald entry points: rebuild it (__graft_entry__.build())")
         for name, (res, args) in _SIGNATURES.items():
             fn = getattr(handle, name)
             fn.restype = res

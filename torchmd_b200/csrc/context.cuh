@@ -136,7 +136,9 @@ struct PairParams64 {
   int has_cutoff, has_switch, rfa, true_gradient;
   double s_max;        // largest double s with sqrt_rn(s) <= cutoff; +inf without cutoff
   double cutoff, switch_dist, inv_sw_width;  // 1 / (cutoff - switch_dist)
-  double krf, crf;     // reaction-field constants (forces.py:466-468)
+  // reaction-field constants (forces.py:466-468), or with particle-mesh Ewald alpha and 2 alpha / sqrt(pi)
+  union { double krf; double ew_alpha; };
+  union { double crf; double ew_beta; };
 };
 struct DeviceState64 {
   Rec64* xq_s;         // [rep*(natoms+1) + k] sorted records; record natoms is the NaN sentinel
@@ -171,6 +173,7 @@ struct tmd_ctx {
   double coulomb = 0.0, cutoff = -1.0, switch_dist = -1.0, skin = 0.0;
   int rfa = 0;
   bool have_atoms = false, have_nonbonded = false, have_box = false, have_excl = false;
+  bool excl_is_set = true;           // the exclusion CSR lists every pair in both rows, once, and no atom with itself
   bool periodic = false;
   bool safe_image = false;           // guard-free minimum image valid (see min_image_fast)
   int coop_blocks = 0;               // CTAs per replica of the cooperative rebuild kernel (0: separate kernels)

@@ -70,7 +70,9 @@ __device__ __forceinline__ double pair_s64(const Rec64& a, const Rec64& b, doubl
 }
 
 // dE/dr of one in-cutoff pair summed over the enabled terms (forces.py:381-491 in fp64); the
-// per-term energies are ADDED to e_*.
+// per-term energies are ADDED to e_*.  EWALD: electrostatics as the real-space part of particle-mesh
+// Ewald, qq erfc(alpha r) / r.
+template <bool EWALD>
 __device__ __forceinline__ double pair_terms64(const PairParams64& pp, double s, double qq, double A, double B, double& e_el,
                                                double& e_lj, double& e_rep, double& e_cg, double& rinv) {
   const double r = sqrt_rn(s);
@@ -98,7 +100,12 @@ __device__ __forceinline__ double pair_terms64(const PairParams64& pp, double s,
     dedr += f;
   }
   if (pp.terms & T_ELEC) {
-    if (pp.rfa) {
+    if (EWALD) {
+      const double ar = pp.ew_alpha * r;
+      const double e = qq * erfc(ar) * rinv;
+      e_el += e;
+      dedr -= (e + qq * pp.ew_beta * exp(-ar * ar)) * rinv;
+    } else if (pp.rfa) {
       e_el += qq * (rinv + pp.krf * s - pp.crf);
       dedr += qq * (2.0 * pp.krf * r - rinv2);
     } else {
@@ -118,9 +125,9 @@ __device__ __forceinline__ double pair_terms64(const PairParams64& pp, double s,
   return dedr;
 }
 
-template <bool ENERGY, bool PERIODIC>
-__global__ void __launch_bounds__(PAIR_WARPS * 32)
-k_pair_f64(DeviceState S, DeviceState64 D, double* __restrict__ forces, double* __restrict__ energies) {
+template <bool ENERGY, bool PERIODIC, bool EWALD>
+__device__ __forceinline__ void pair_f64_body(const DeviceState& S, const DeviceState64& D, double* __restrict__ forces,
+                                              double* __restrict__ energies) {
   const int r = blockIdx.y;
   const int lane = threadIdx.x & 31;
   const int k = blockIdx.x * PAIR_WARPS + (threadIdx.x >> 5);
@@ -157,7 +164,7 @@ k_pair_f64(DeviceState S, DeviceState64 D, double* __restrict__ forces, double* 
         B = D.AB[t + 1];
       }
       double rinv;
-      const double dedr = pair_terms64(pp, s, pi.q * pj.q, A, B, e_el, e_lj, e_rep, e_cg, rinv);
+      const double dedr = pair_terms64<EWALD>(pp, s, pi.q * pj.q, A, B, e_el, e_lj, e_rep, e_cg, rinv);
       const double c = dedr * rinv;
       fx -= wx * c;
       fy -= wy * c;
@@ -181,6 +188,17 @@ k_pair_f64(DeviceState S, DeviceState64 D, double* __restrict__ forces, double* 
     if (pp.terms & T_REP) block_accumulate<PAIR_WARPS>(0.5 * e_rep, E + TMD_E_REPULSION, red);
     if (pp.terms & T_REPCG) block_accumulate<PAIR_WARPS>(0.5 * e_cg, E + TMD_E_REPULSIONCG, red);
   }
+}
+template <bool ENERGY, bool PERIODIC>
+__global__ void __launch_bounds__(PAIR_WARPS * 32)
+k_pair_f64(DeviceState S, DeviceState64 D, double* __restrict__ forces, double* __restrict__ energies) {
+  pair_f64_body<ENERGY, PERIODIC, false>(S, D, forces, energies);
+}
+// particle-mesh Ewald contexts (periodic only): the same rows with the real-space Ewald electrostatics
+template <bool ENERGY>
+__global__ void __launch_bounds__(PAIR_WARPS * 32)
+k_ewpair64(DeviceState S, DeviceState64 D, double* __restrict__ forces, double* __restrict__ energies) {
+  pair_f64_body<ENERGY, true, true>(S, D, forces, energies);
 }
 
 // k_export_pairs with the fp64 decision.

@@ -53,7 +53,8 @@ __device__ __forceinline__ void block_accumulate(double v, double* dst, double* 
 
 // ENERGY   also accumulate the per-term energies (only the last step of a fused run needs them)
 // PERIODIC minimum image on; SAFE: guard-free minimum image (see min_image_fast)
-// MODE     0 = pair terms selected at run time, 1 = LJ+switch + reaction-field Coulomb
+// MODE     0 = pair terms selected at run time, 1 = LJ+switch + reaction-field Coulomb,
+//          2 = pair terms selected at run time with real-space Ewald electrostatics (particle-mesh Ewald)
 template <bool ENERGY, bool PERIODIC, bool SAFE, int MODE>
 __global__ void __launch_bounds__(PAIR_WARPS * 32, PAIR_MINBLOCKS)
 k_pair(DeviceState S, float* __restrict__ forces, double* __restrict__ energies) {
@@ -363,9 +364,9 @@ __device__ __forceinline__ void lj_pair_entries(smem_addr ab_row, const float2* 
   }
 }
 
-template <bool ENERGY, bool SMALLT>
-__global__ void __launch_bounds__(PAIR_WARPS * 32, PAIR_FX2_MINBLOCKS)
-k_pair_fx2(DeviceState S, SwitchConsts sc, float* __restrict__ forces, double* __restrict__ energies) {
+template <bool ENERGY, bool SMALLT, bool EW>
+__device__ __forceinline__ void pair_fx2_body(const DeviceState& S, const SwitchConsts& sc, float* __restrict__ forces,
+                                              double* __restrict__ energies) {
   const int r = blockIdx.y;
   const int lane = threadIdx.x & 31;
   const int kk = blockIdx.x * PAIR_WARPS + (threadIdx.x >> 5);
@@ -430,8 +431,8 @@ k_pair_fx2(DeviceState S, SwitchConsts sc, float* __restrict__ forces, double* _
       lj_pair_entries<SMALLT>(ab_row, ab_global, (S.pp.terms & T_LJ) != 0, en0, en1, A, B);
       const F2 nqq = f2_mul(f2(nqi), f2(__int_as_float(p0.w), __int_as_float(p1.w)));
       F2 elj, neel;
-      F2 nc = pair_coef2<ENERGY>(sc, s, nqq, A, B, f2(rsqrt_seed(s.x), rsqrt_seed(s.y)),
-                                 f2(neg_rcp_seed(s.x), neg_rcp_seed(s.y)), elj, neel);
+      F2 nc = pair_coef2<ENERGY, EW>(sc, s, nqq, A, B, f2(rsqrt_seed(s.x), rsqrt_seed(s.y)),
+                                     f2(neg_rcp_seed(s.x), neg_rcp_seed(s.y)), elj, neel);
       nc = f2(in0 ? nc.x : 0.f, in1 ? nc.y : 0.f);  // a select, not a product: the other half may hold inf/NaN
       FX = f2_fma(wx, nc, FX);
       FY = f2_fma(wy, nc, FY);
@@ -512,7 +513,7 @@ k_pair_fx2(DeviceState S, SwitchConsts sc, float* __restrict__ forces, double* _
                        pp.s_max)) {
           const float2 ab = __ldg(S.AB + ti + (entry >> 24));  // (pair_terms<0> ignores it when LJ is off)
           float rinv;
-          const float dedr = pair_terms<0>(pp, s, qi * __int_as_float(pj.w), ab.x, ab.y, e_el, e_lj, e_rep, e_cg, rinv);
+          const float dedr = pair_terms<EW ? 2 : 0>(pp, s, qi * __int_as_float(pj.w), ab.x, ab.y, e_el, e_lj, e_rep, e_cg, rinv);
           const float c = dedr * rinv;
           fx -= wx * c;
           fy -= wy * c;
@@ -537,6 +538,17 @@ k_pair_fx2(DeviceState S, SwitchConsts sc, float* __restrict__ forces, double* _
     block_accumulate<PAIR_WARPS>(0.5 * (double)e_el, E + TMD_E_ELECTROSTATICS, red);  // every pair is seen from both atoms
     block_accumulate<PAIR_WARPS>(0.5 * (double)e_lj, E + TMD_E_LJ, red);
   }
+}
+template <bool ENERGY, bool SMALLT>
+__global__ void __launch_bounds__(PAIR_WARPS * 32, PAIR_FX2_MINBLOCKS)
+k_pair_fx2(DeviceState S, SwitchConsts sc, float* __restrict__ forces, double* __restrict__ energies) {
+  pair_fx2_body<ENERGY, SMALLT, false>(S, sc, forces, energies);
+}
+// particle-mesh Ewald contexts: real-space Ewald electrostatics (sc from make_switch_consts_ewald)
+template <bool ENERGY, bool SMALLT>
+__global__ void __launch_bounds__(PAIR_WARPS * 32, PAIR_FX2_MINBLOCKS)
+k_pair_fx2_ew(DeviceState S, SwitchConsts sc, float* __restrict__ forces, double* __restrict__ energies) {
+  pair_fx2_body<ENERGY, SMALLT, true>(S, sc, forces, energies);
 }
 
 // ---- systems without a box: fp32x2 arithmetic on the float records -------------------------

@@ -302,7 +302,10 @@ struct PairParams {
   float cutoff;       // fl32(cutoff)
   float switch_dist;  // fl32(switch_dist)
   float inv_sw_width; // 1 / (cutoff - switch_dist)
-  float krf, crf;     // reaction-field constants (forces.py:466-468)
+  // reaction-field constants (forces.py:466-468); with particle-mesh Ewald, which excludes the reaction field, the same
+  // words hold the Ewald splitting parameter alpha and 2 alpha / sqrt(pi)
+  union { float krf; float ew_alpha; };
+  union { float crf; float ew_beta; };
   float two_krf;
   int true_gradient;  // 1: switched-LJ force is the exact d(E*s)/dr (the reference's autograd path, forces.py:328-336);
                       // 0: the reference's explicit formula with its extra 1/r (forces.py:410-412)
@@ -322,7 +325,11 @@ enum : uint32_t {
 // e_rep / e_repcg.  Follows forces.py:381-491 including the reference's switched
 // LJ force  s*dE/dr + E*s'/r  (the extra 1/r is the reference's, forces.py:410-412).
 // MODE 0: terms chosen at run time from pp;  MODE 1: LJ with switch + reaction-field
-// electrostatics (the production water/protein set-up) resolved at compile time.
+// electrostatics (the production water/protein set-up) resolved at compile time;  MODE 2: terms
+// chosen at run time, electrostatics as the real-space part of particle-mesh Ewald,
+// qq erfc(alpha r) / r with no shift or switch.  erfcf and expf are the CUDA library functions
+// (at most 4 and 2 ulp: CUDA C Programming Guide, "Mathematical Functions"), so a pair's energy and
+// force coefficient are within about 1e-6 relative of their exact values.
 template <int MODE>
 TMD_HD float pair_terms(const PairParams& pp, float s, float qq, float A, float B,
                         float& e_el, float& e_lj, float& e_rep, float& e_repcg,
@@ -358,7 +365,12 @@ TMD_HD float pair_terms(const PairParams& pp, float s, float qq, float A, float 
     dedr += f;
   }
   if (do_el) {
-    if (rf_on) {
+    if (MODE == 2) {
+      const float ar = pp.ew_alpha * r;
+      const float e = qq * erfcf(ar) * rinv;
+      e_el += e;
+      dedr -= (e + qq * pp.ew_beta * expf(-ar * ar)) * rinv;
+    } else if (rf_on) {
       e_el += qq * (rinv + pp.krf * s - pp.crf);
       dedr += qq * (pp.two_krf * r - rinv2);
     } else {
@@ -411,7 +423,8 @@ TMD_HD float neg_rcp_seed(float s) {
 struct SwitchConsts {
   float neg_switch_dist, inv_sw_width;
   float d1, d2, d3;  // -ds/dr polynomial: t^2 (d3 + t (d2 + t d1)),  d = (30, -60, 30) / (cutoff - switch_dist)
-  float two_krf, krf, neg_crf;
+  float two_krf, krf, neg_crf;  // reaction field; the Ewald variants (EW) read 2 alpha / sqrt(pi) and alpha from the
+                                // first two (the reaction field and PME exclude each other; make_switch_consts_ewald)
 };
 // Also covers the term sets without switching (t stays 0: sw = 1, ds/dr = 0) and without a reaction field
 // (k_rf = c_rf = 0: plain Coulomb), so pair_coef2 serves every combination of "lj" and "electrostatics".
@@ -433,6 +446,25 @@ inline SwitchConsts make_switch_consts(const PairParams& pp) {
   c.neg_crf = pp.rfa ? -pp.crf : 0.0f;
   return c;
 }
+// The Ewald instantiations (EW) of pair_coef2 and the cluster kernel's coefficient read alpha and 2 alpha / sqrt(pi).
+inline SwitchConsts make_switch_consts_ewald(const PairParams& pp) {
+  SwitchConsts c = make_switch_consts(pp);
+  c.two_krf = pp.ew_beta;
+  c.krf = pp.ew_alpha;
+  c.neg_crf = 0.0f;
+  return c;
+}
+
+// Real-space Ewald electrostatics of two partners for the packed coefficients: MINUS dE/dr and MINUS the energy,
+//   -dE/dr = nqq (erfc(alpha r) (-1/r^2) - beta exp(-alpha^2 r^2) / r),   -E = nqq erfc(alpha r) / r
+// with nqq = -(k qi qj) and nr2 = -1/r^2 (erfcf / expf per half, within 4 / 2 ulp).
+TMD_HD F2 ewald_ndedr2(const SwitchConsts& c, F2 nqq, F2 r, F2 rinv, F2 nr2, F2& erfc_ar) {
+  const F2 ar = f2_mul(r, f2(c.krf));  // alpha
+  erfc_ar = f2(erfcf(ar.x), erfcf(ar.y));
+  const F2 ex = f2(expf(-ar.x * ar.x), expf(-ar.y * ar.y));
+  const F2 nb = f2_mul(f2_mul(ex, rinv), f2(-c.two_krf));  // -2 alpha / sqrt(pi) exp(-alpha^2 r^2) / r
+  return f2_mul(nqq, f2_fma(erfc_ar, nr2, nb));
+}
 
 // MINUS the force coefficient (dE/dr)/r of two partners for LJ with switch + reaction-field
 // Coulomb in the explicit-force convention (pair_terms<1> restated with packed operations and
@@ -441,7 +473,8 @@ inline SwitchConsts make_switch_consts(const PairParams& pp) {
 //   y    rsqrt_seed(s)              nz   neg_rcp_seed(s)
 // The force on atom i is then  F_i += w * result.  ENERGY: also the switched LJ energy and MINUS the
 // reaction-field Coulomb energy of each partner (forces.py:389-415, 466-478).
-template <bool ENERGY>
+// EW: real-space Ewald electrostatics (ewald_ndedr2) in place of the reaction field.
+template <bool ENERGY, bool EW = false>
 TMD_HD F2 pair_coef2(const SwitchConsts& c, F2 s, F2 nqq, F2 A, F2 B, F2 y, F2 nz, F2& e_lj, F2& ne_el) {
   // 1/r to ~1 ulp and r
   const F2 t = f2_mul(s, y);
@@ -466,6 +499,15 @@ TMD_HD F2 pair_coef2(const SwitchConsts& c, F2 s, F2 nqq, F2 A, F2 B, F2 y, F2 n
   // -(s dE/dr + E s'/r)   (the reference's explicit formula, forces.py:410-412)
   const F2 nfsw = f2_fma(sw, nf, f2_mul(f2_mul(e, ndsw), rinv));
   // reaction field: dE/dr = qq (2 k_rf r - 1/r^2)
+  if constexpr (EW) {
+    F2 ec;
+    const F2 ndedr = f2_add(ewald_ndedr2(c, nqq, r, rinv, nr2, ec), nfsw);
+    if (ENERGY) {
+      e_lj = f2_mul(e, sw);
+      ne_el = f2_mul(f2_mul(nqq, ec), rinv);  // -qq erfc(alpha r) / r
+    }
+    return f2_mul(ndedr, rinv);
+  }
   const F2 ndedr = f2_fma(nqq, f2_fma(f2(c.two_krf), r, nr2), nfsw);
   if (ENERGY) {
     e_lj = f2_mul(e, sw);

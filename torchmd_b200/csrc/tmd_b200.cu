@@ -23,6 +23,7 @@
 #include "fused.cuh"
 #include "double.cuh"
 #include "constrain.cuh"
+#include "pme.cuh"
 
 using namespace tmd;
 
@@ -211,6 +212,15 @@ struct CtxPriv {
   void* con_ref = nullptr;   // (R,N,3) positions before the drift, in the context's precision
   int* con_fail = nullptr;   // a group's SHAKE iteration did not converge (tmd_get_stats reports it)
   const void* con_pos = nullptr;  // positions of the last tmd_vv_first[_f64]: what tmd_vv_second[_f64] constrains against
+  // tmd_set_pme: particle-mesh Ewald (pme.cuh); pme_tol <= 0 means off.  alpha and the grid are chosen by pme_choose.
+  double pme_tol = 0.0, pme_alpha = 0.0;
+  int pme_K[3] = {0, 0, 0};
+  PmeArgs pme{};  // the reciprocal kernels' arguments (buffers below, owned)
+  double *pme_q = nullptr, *pme_L = nullptr, *pme_tw = nullptr, *pme_econst = nullptr;
+  unsigned long long* pme_qgrid = nullptr;
+  void *pme_cgrid = nullptr, *pme_infl = nullptr;
+  cudaStream_t pme_side = nullptr;  // fp32: the reciprocal chain runs here, beside the pair kernel
+  cudaEvent_t pme_fork = nullptr, pme_join = nullptr;
 };
 
 }  // namespace
@@ -228,6 +238,47 @@ static int need_precision(tmd_ctx* ctx, int bits, const char* name) {
 }
 #define TMD_PRECISION(ctx, bits, name) \
   if (int rc__ = need_precision((ctx), (bits), (name))) return rc__;
+
+// ---- particle-mesh Ewald: parameter choice (the one place it is made) ------------------------
+static inline bool pme_on(tmd_ctx* ctx) { return priv(ctx).pme_tol > 0.0; }
+// MODE of the full-row pair kernels (physics.cuh, pair_terms): a PME context never runs another
+static int pair_mode_of(tmd_ctx* ctx) {
+  if (pme_on(ctx)) return 2;
+  return (ctx->pair_mask == (T_LJ | T_ELEC) && ctx->d.pp.has_switch && ctx->d.pp.rfa && !ctx->exact_gradient) ? 1 : 0;
+}
+static int smallest_235(int n) {
+  for (int m = std::max(n, 1);; ++m) {
+    int k = m;
+    for (int p : {2, 3, 5})
+      while (k % p == 0) k /= p;
+    if (k == 1) return m;
+  }
+}
+// alpha = sqrt(-ln 2 tol) / rc; n_d = smallest 2^a 3^b 5^c >= max(2 alpha L_d / (3 tol^(1/5)), 10), the largest over
+// the replicas (OpenMM's choice).  The real-space sum is a minimum-image sum, so every box must be at least two
+// cutoffs long on every axis; the line kernels hold at most PME_MAX_N points.
+static int pme_choose(tmd_ctx* ctx, double tol, const double* box, double* alpha, int K[3]) {
+  if (ctx->cutoff < 0) return fail(TMD_ERR_UNSUPPORTED, "particle-mesh Ewald needs a cutoff");
+  const double rc = ctx->cutoff;
+  *alpha = sqrt(-log(2.0 * tol)) / rc;
+  for (int d = 0; d < 3; ++d) {
+    double lmax = 0.0;
+    for (int r = 0; r < ctx->nrep; ++r) {
+      const double L = box[3 * r + d];
+      if (!(L > 0.0)) return fail(TMD_ERR_UNSUPPORTED, "particle-mesh Ewald needs a periodic box on every replica");
+      if (rc > 0.5 * L)
+        return fail(TMD_ERR_UNSUPPORTED, "particle-mesh Ewald needs cutoff <= half of every box length (the real-space "
+                                         "sum takes the minimum image only)");
+      lmax = std::max(lmax, L);
+    }
+    const double want = std::max(2.0 * *alpha * lmax / (3.0 * pow(tol, 0.2)), 10.0);
+    K[d] = smallest_235((int)std::min(ceil(want), 1e6));
+    if (K[d] > PME_MAX_N)
+      return fail(TMD_ERR_UNSUPPORTED, "particle-mesh Ewald grid of " + std::to_string(K[d]) + " points along an axis: the FFT "
+                                       "kernels take at most " + std::to_string(PME_MAX_N) + " (a larger tolerance or smaller box)");
+  }
+  return TMD_OK;
+}
 // ---- peer-to-peer position exchange --------------------------------------------------------
 static inline float* dd_pos_of(tmd_ctx* ctx, int peer, int which) {
   return reinterpret_cast<float*>(static_cast<char*>(ctx->dd_peer_base[peer]) + (size_t)which * ctx->dd_pos_bytes);
@@ -253,7 +304,7 @@ const char* tmd_last_error(void) { return g_err.c_str(); }
 #if defined(TMD_SIMT_HOST)
 int tmd_version(void) { return -100; }  // host SIMT interpreter build (tests/simt): torchmd_b200/_lib.py refuses it
 #else
-int tmd_version(void) { return 102; }  // 101: the "precision: double" entry points (tmd_set_precision, *_f64); 102: constraints
+int tmd_version(void) { return 103; }  // 101: the "precision: double" entry points (tmd_set_precision, *_f64); 102: constraints; 103: PME
 #endif
 
 int tmd_create(tmd_ctx** out, int device, int natoms, int nreplicas) {
@@ -338,6 +389,14 @@ int tmd_destroy(tmd_ctx* ctx) {
   if (priv(ctx).bonded_scratch) cudaFree(priv(ctx).bonded_scratch);
   for (void* b : {(void*)priv(ctx).con_groups, (void*)priv(ctx).con_free, (void*)priv(ctx).con_L, priv(ctx).con_ref, (void*)priv(ctx).con_fail})
     if (b) cudaFree(b);
+  {
+    CtxPriv& p = priv(ctx);
+    for (void* b : {(void*)p.pme_q, (void*)p.pme_L, (void*)p.pme_tw, (void*)p.pme_econst, (void*)p.pme_qgrid, p.pme_cgrid, p.pme_infl})
+      if (b) cudaFree(b);
+    if (p.pme_side) cudaStreamDestroy(p.pme_side);
+    if (p.pme_fork) cudaEventDestroy(p.pme_fork);
+    if (p.pme_join) cudaEventDestroy(p.pme_join);
+  }
   delete static_cast<tmd_ctx_full*>(ctx);
   return TMD_OK;
 }
@@ -376,6 +435,17 @@ int tmd_set_exclusions(tmd_ctx* ctx, const int64_t* row_ptr, const int32_t* cols
   if ((rc = upload(&ctx->excl_ptr, rp.data(), rp.size()))) return rc;
   if ((rc = upload(&ctx->excl_idx, cols, (size_t)row_ptr[n]))) return rc;
   ctx->have_excl = row_ptr[n] > 0;
+  {  // particle-mesh Ewald reads the rows as the set of excluded pairs (pme_finalize refuses anything else)
+    std::vector<std::pair<int, int>> e;
+    e.reserve((size_t)row_ptr[n]);
+    for (int i = 0; i < n; ++i)
+      for (int64_t k = row_ptr[i]; k < row_ptr[i + 1]; ++k) e.emplace_back(i, cols[k]);
+    std::sort(e.begin(), e.end());
+    bool ok = std::adjacent_find(e.begin(), e.end()) == e.end();
+    for (size_t k = 0; ok && k < e.size(); ++k)
+      ok = e[k].first != e[k].second && std::binary_search(e.begin(), e.end(), std::make_pair(e[k].second, e[k].first));
+    ctx->excl_is_set = ok;
+  }
   ctx->touched = true;
   priv(ctx).dirty = true;
   return TMD_OK;
@@ -567,6 +637,14 @@ static int set_box(tmd_ctx* ctx, const T* box_diag) {
   }
   if (nzero != 0 && nzero != ctx->nrep * 3)
     return fail(TMD_ERR_UNSUPPORTED, "tmd_set_box: box must be all zero (no wrapping) or all positive");
+  if (pme_on(ctx)) {  // alpha and the grid follow the box
+    std::vector<double> b(box_diag, box_diag + ctx->nrep * 3);
+    double alpha;
+    int K[3];
+    if (int rc = pme_choose(ctx, priv(ctx).pme_tol, b.data(), &alpha, K)) return fail(rc, "tmd_set_box: " + g_err);
+    priv(ctx).pme_alpha = alpha;
+    for (int d = 0; d < 3; ++d) priv(ctx).pme_K[d] = K[d];
+  }
   ctx->periodic = (nzero == 0);
   ctx->box_host.assign(box_diag, box_diag + ctx->nrep * 3);
   ctx->box64_host.assign(box_diag, box_diag + ctx->nrep * 3);
@@ -588,10 +666,188 @@ int tmd_set_box_f64(tmd_ctx* ctx, const double* box_diag) {
   return set_box(ctx, box_diag);
 }
 
+// ---- particle-mesh Ewald ----------------------------------------------------------------------
+int tmd_set_pme(tmd_ctx* ctx, double tolerance) {
+  if (!ctx) return fail(TMD_ERR_ARG, "tmd_set_pme: null context");
+  CtxPriv& pv = priv(ctx);
+  if (!(tolerance > 0.0)) {
+    if (pme_on(ctx)) {
+      pv.pme_tol = 0.0;
+      if (!ctx->rfa) {  // (the reaction-field words held the Ewald constants)
+        ctx->d.pp.krf = ctx->d.pp.crf = 0.f;
+        ctx->d64.pp.krf = ctx->d64.pp.crf = 0.0;
+      }
+      pv.dirty = true;
+    }
+    return TMD_OK;
+  }
+  if (!(tolerance < 0.5)) return fail(TMD_ERR_ARG, "tmd_set_pme: the tolerance must be below 0.5");
+  if (ctx->dd_base || !ctx->d.own_all)
+    return fail(TMD_ERR_UNSUPPORTED, "tmd_set_pme: decomposed runs cannot use particle-mesh Ewald");
+  if (!ctx->have_nonbonded) return fail(TMD_ERR_STATE, "tmd_set_pme: call tmd_set_nonbonded first");
+  if (ctx->cutoff < 0) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_pme: particle-mesh Ewald needs a cutoff");
+  if (ctx->rfa) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_pme: particle-mesh Ewald and the reaction field exclude each other");
+  if (!(ctx->pair_mask & T_ELEC)) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_pme: particle-mesh Ewald needs the electrostatics term");
+  if (ctx->have_box) {
+    double alpha;
+    int K[3];
+    if (!ctx->periodic) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_pme: particle-mesh Ewald needs a periodic box on every replica");
+    if (int rc = pme_choose(ctx, tolerance, ctx->box64_host.data(), &alpha, K)) return fail(rc, "tmd_set_pme: " + g_err);
+    pv.pme_alpha = alpha;
+    for (int d = 0; d < 3; ++d) pv.pme_K[d] = K[d];
+  }
+  pv.pme_tol = tolerance;
+  ctx->touched = true;
+  pv.dirty = true;
+  return TMD_OK;
+}
+
+int tmd_get_pme(tmd_ctx* ctx, double* alpha, int32_t grid[3]) {
+  if (!ctx || !alpha || !grid) return fail(TMD_ERR_ARG, "tmd_get_pme: bad arguments");
+  if (!pme_on(ctx)) return fail(TMD_ERR_STATE, "tmd_get_pme: particle-mesh Ewald is off (tmd_set_pme)");
+  if (!ctx->have_box) return fail(TMD_ERR_STATE, "tmd_get_pme: the grid follows the box: call tmd_set_box first");
+  *alpha = priv(ctx).pme_alpha;
+  for (int d = 0; d < 3; ++d) grid[d] = priv(ctx).pme_K[d];
+  return TMD_OK;
+}
+
 }  // extern "C"
 
 // ---- finalise: host-side sizing, allocation, uploads (first use / after changes) ----------
 static constexpr double F64_POS_LIMIT = 8192.0;  // A: fp64 contexts flag coordinates from here on (margin, finalize)
+
+// Particle-mesh Ewald tables of the context's boxes: the pair kernels' Ewald constants, twiddles, the influence function
+// G(m) with the B-spline moduli, the self + background energies, and the grids.
+static int pme_finalize(tmd_ctx* ctx) {
+  CtxPriv& pv = priv(ctx);
+  if (!ctx->periodic) return fail(TMD_ERR_UNSUPPORTED, "particle-mesh Ewald needs a periodic box on every replica");
+  if (ctx->rfa) return fail(TMD_ERR_UNSUPPORTED, "particle-mesh Ewald and the reaction field exclude each other");
+  if (!(ctx->pair_mask & T_ELEC)) return fail(TMD_ERR_UNSUPPORTED, "particle-mesh Ewald needs the electrostatics term");
+  if (!ctx->excl_is_set)
+    return fail(TMD_ERR_ARG, "particle-mesh Ewald: tmd_set_exclusions must list every excluded pair in both rows, once, "
+                             "and no atom with itself (the exclusion correction sums each row)");
+  double alpha;
+  int K[3];
+  if (int rc = pme_choose(ctx, pv.pme_tol, ctx->box64_host.data(), &alpha, K)) return rc;
+  pv.pme_alpha = alpha;
+  for (int d = 0; d < 3; ++d) pv.pme_K[d] = K[d];
+  const double beta = 2.0 * alpha / sqrt(M_PI);
+  ctx->d.pp.ew_alpha = (float)alpha;
+  ctx->d.pp.ew_beta = (float)beta;
+  ctx->d64.pp.ew_alpha = alpha;
+  ctx->d64.pp.ew_beta = beta;
+  const int N = ctx->natoms, R = ctx->nrep;
+  const bool f64 = ctx->precision == 64;
+  const size_t ktot = (size_t)K[0] * K[1] * K[2];
+  int rc;
+  // charges carry sqrt(coulomb constant), as in the pair kernels
+  std::vector<double> q(N);
+  const double sk = sqrt(ctx->coulomb > 0 ? ctx->coulomb : 0.0);
+  double qabs = 0.0, qsum = 0.0, q2 = 0.0;
+  for (int i = 0; i < N; ++i) {
+    q[i] = (f64 ? ctx->charges64_host[i] : (double)ctx->charges_host[i]) * sk;
+    qabs += fabs(q[i]);
+    qsum += q[i];
+    q2 += q[i] * q[i];
+  }
+  // Fixed point of the charge grid: a point receives q th_x th_y th_z from at most every atom, and the weights of one
+  // atom sum to 1, so |value| <= sum |q| over the whole grid.  scale = 2^e with e the largest integer such that
+  // scale * sum|q| <= 2^61; each contribution rounds by at most 1/2 unit, 125 per atom, so the integer sum stays below
+  // 2^61 + 63 N < 2^63 for any N < 2^55.  Resolution 2^-e, e.g. 2^-40 e for 10^5 TIP3P atoms.
+  const double e = qabs > 0.0 ? floor(61.0 - log2(qabs)) : 40.0;
+  const double scale = ldexp(1.0, (int)std::min(e, 1000.0));
+  std::vector<double> tw(2 * (size_t)(K[0] + K[1] + K[2]));
+  {
+    size_t o = 0;
+    for (int d = 0; d < 3; ++d)
+      for (int t = 0; t < K[d]; ++t, ++o) {
+        tw[2 * o] = cos(2.0 * M_PI * t / K[d]);
+        tw[2 * o + 1] = -sin(2.0 * M_PI * t / K[d]);
+      }
+  }
+  // |b(m)|^2 of order-5 B-splines (zeros at m = K/2 take their neighbours' mean, as OpenMM does)
+  double th[PME_ORDER], dth[PME_ORDER];
+  pme_bspline(0.0, th, dth);
+  std::vector<double> mod[3];
+  for (int d = 0; d < 3; ++d) {
+    mod[d].resize(K[d]);
+    for (int m = 0; m < K[d]; ++m) {
+      double re = 0.0, im = 0.0;
+      for (int k = 0; k < PME_ORDER; ++k) {
+        re += th[k] * cos(2.0 * M_PI * m * k / K[d]);
+        im += th[k] * sin(2.0 * M_PI * m * k / K[d]);
+      }
+      mod[d][m] = re * re + im * im;
+    }
+    for (int m = 0; m < K[d]; ++m)
+      if (mod[d][m] < 1e-7) mod[d][m] = 0.5 * (mod[d][(m + K[d] - 1) % K[d]] + mod[d][(m + 1) % K[d]]);
+  }
+  std::vector<double> G((size_t)R * ktot), econst(R);
+  for (int r = 0; r < R; ++r) {
+    const double* L = &ctx->box64_host[3 * r];
+    const double V = L[0] * L[1] * L[2];
+    econst[r] = -alpha / sqrt(M_PI) * q2 - M_PI * qsum * qsum / (2.0 * V * alpha * alpha);
+    for (int x = 0; x < K[0]; ++x) {
+      const double mx = (x > K[0] / 2 ? x - K[0] : x) / L[0];
+      for (int y = 0; y < K[1]; ++y) {
+        const double my = (y > K[1] / 2 ? y - K[1] : y) / L[1];
+        for (int z = 0; z < K[2]; ++z) {
+          const double mz = (z > K[2] / 2 ? z - K[2] : z) / L[2];
+          const double m2 = mx * mx + my * my + mz * mz;
+          const size_t idx = (size_t)r * ktot + ((size_t)x * K[1] + y) * K[2] + z;
+          G[idx] = m2 > 0.0 ? exp(-M_PI * M_PI * m2 / (alpha * alpha)) / (M_PI * V * m2 * mod[0][x] * mod[1][y] * mod[2][z]) : 0.0;
+        }
+      }
+    }
+  }
+  for (void* b : {(void*)pv.pme_qgrid, pv.pme_cgrid, pv.pme_infl})
+    if (b) cudaFree(b);
+  pv.pme_qgrid = nullptr;
+  pv.pme_cgrid = nullptr;
+  pv.pme_infl = nullptr;
+  if ((rc = upload(&pv.pme_q, q.data(), q.size()))) return rc;
+  if ((rc = upload(&pv.pme_L, ctx->box64_host.data(), ctx->box64_host.size()))) return rc;
+  if ((rc = upload(&pv.pme_tw, tw.data(), tw.size()))) return rc;
+  if ((rc = upload(&pv.pme_econst, econst.data(), econst.size()))) return rc;
+  if ((rc = device_alloc(&pv.pme_qgrid, (size_t)R * ktot))) return rc;
+  TMD_CUDA(cudaMemset(pv.pme_qgrid, 0, (size_t)R * ktot * sizeof(unsigned long long)));
+  if (f64) {
+    if ((rc = upload(reinterpret_cast<double**>(&pv.pme_infl), G.data(), G.size()))) return rc;
+    if ((rc = device_alloc(reinterpret_cast<Cplx<double>**>(&pv.pme_cgrid), (size_t)R * ktot))) return rc;
+  } else {
+    std::vector<float> g32(G.begin(), G.end());
+    if ((rc = upload(reinterpret_cast<float**>(&pv.pme_infl), g32.data(), g32.size()))) return rc;
+    if ((rc = device_alloc(reinterpret_cast<Cplx<float>**>(&pv.pme_cgrid), (size_t)R * ktot))) return rc;
+    if (!pv.pme_side) {
+      TMD_CUDA(cudaStreamCreateWithFlags(&pv.pme_side, cudaStreamNonBlocking));
+      TMD_CUDA(cudaEventCreateWithFlags(&pv.pme_fork, cudaEventDisableTiming));
+      TMD_CUDA(cudaEventCreateWithFlags(&pv.pme_join, cudaEventDisableTiming));
+    }
+  }
+  PmeArgs& a = pv.pme;
+  a.natoms = N;
+  for (int d = 0; d < 3; ++d) a.K[d] = K[d];
+  a.ktot = (long long)ktot;
+  a.scale = scale;
+  a.inv_scale = 1.0 / scale;
+  a.q = pv.pme_q;
+  a.L = pv.pme_L;
+  a.qgrid = pv.pme_qgrid;
+  a.cgrid = pv.pme_cgrid;
+  a.tw = pv.pme_tw;
+  a.infl = pv.pme_infl;
+  a.econst = pv.pme_econst;
+  a.excl_ptr = ctx->have_excl ? ctx->excl_ptr : nullptr;
+  a.excl_idx = ctx->have_excl ? ctx->excl_idx : nullptr;
+  a.alpha = alpha;
+  a.beta = beta;
+  const ClusterState& cl = ctx->d.cl;
+  a.cl_f = cl.on ? cl.f : nullptr;
+  a.cl_inv = cl.on ? cl.inv : nullptr;
+  a.cl_stride = (long long)cl.slots + 1;
+  return TMD_OK;
+}
+
 static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   if (!ctx->have_atoms) return fail(TMD_ERR_STATE, "tmd_set_atoms has not been called");
   if (!ctx->have_box) return fail(TMD_ERR_STATE, "tmd_set_box has not been called");
@@ -714,7 +970,7 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   }
   d.check_far = ctx->safe_image ? 1 : 0;
   d.pp.true_gradient = ctx->exact_gradient;
-  ctx->pair_mode = (ctx->pair_mask == (T_LJ | T_ELEC) && d.pp.has_switch && d.pp.rfa && !ctx->exact_gradient) ? 1 : 0;
+  ctx->pair_mode = pair_mode_of(ctx);
 
   // Fixed-point separations in the pair kernel (k_pair_fx): periodic box with the guard-free
   // image condition (TMD_B200_FX=1 or 2).
@@ -833,8 +1089,9 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
 #if !defined(TMD_SIMT_HOST)
       if (pv.cl_smem > (size_t)180 * 1024) return fail(TMD_ERR_UNSUPPORTED, "cluster lists too long for the shared-memory staging");
       int per_sm = 0;
-      const void* kernels[4] = {(const void*)k_cpair<false, false>, (const void*)k_cpair<false, true>,
-                                (const void*)k_cpair<true, false>, (const void*)k_cpair<true, true>};
+      const void* kernels[6] = {(const void*)k_cpair<false, false>, (const void*)k_cpair<false, true>,
+                                (const void*)k_cpair<true, false>, (const void*)k_cpair<true, true>,
+                                (const void*)k_cpair_ew<false>, (const void*)k_cpair_ew<true>};
       for (const void* k : kernels) TMD_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pv.cl_smem));
       TMD_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cpair<false, true>, CL_WARPS * 32, pv.cl_smem));
       pv.cl_blocks = std::max(1, std::min(ctx->nsm * std::max(per_sm, 1), (cl.nclusters_cap + CL_WARPS - 1) / CL_WARPS));
@@ -974,10 +1231,44 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
     D.pos_limit = has_cut ? F64_POS_LIMIT : INFINITY;  // without a cutoff every pair is listed: nothing to bound
     D.pp.true_gradient = ctx->exact_gradient;
   }
+  if (pme_on(ctx) && (rc = pme_finalize(ctx))) return rc;
   priv(ctx).dirty = false;
   return TMD_OK;
 }
 
+// Particle-mesh Ewald (a periodic box) on the full rows: the real-space Ewald instantiations of the same kernels the
+// context would run without it, and nothing else.  tmd_pair_kernel(): 6 k_pair<MODE 2>, 7 k_pair_fx<MODE 2>,
+// 9 k_pair_fx2_ew (the cluster path: 10 k_cpair_ew).
+static void launch_pair_ewald(tmd_ctx* ctx, dim3 pg, cudaStream_t st, float* forces, double* energies) {
+  const bool e = energies != nullptr, small = ctx->d.ntypes <= FX_SMALLT_MAX;
+  const int th = PAIR_WARPS * 32;
+  const bool lj_el_only = ctx->pair_mask != 0 && (ctx->pair_mask & ~(T_LJ | T_ELEC)) == 0;
+  if (ctx->d.xf_s && ctx->fx_packed && lj_el_only && !ctx->exact_gradient && ctx->d.ntypes <= 128) {
+    ctx->last_pair_kernel = 9;
+    const SwitchConsts sc = make_switch_consts_ewald(ctx->d.pp);
+    if (e && small) launch(k_pair_fx2_ew<true, true>, pg, th, st, ctx->d, sc, forces, energies);
+    else if (e) launch(k_pair_fx2_ew<true, false>, pg, th, st, ctx->d, sc, forces, energies);
+    else if (small) launch(k_pair_fx2_ew<false, true>, pg, th, st, ctx->d, sc, forces, energies);
+    else launch(k_pair_fx2_ew<false, false>, pg, th, st, ctx->d, sc, forces, energies);
+    return;
+  }
+  if (ctx->d.xf_s) {
+    ctx->last_pair_kernel = 7;
+    if (e && small) launch(k_pair_fx<true, 2, true>, pg, th, st, ctx->d, forces, energies);
+    else if (e) launch(k_pair_fx<true, 2, false>, pg, th, st, ctx->d, forces, energies);
+    else if (small) launch(k_pair_fx<false, 2, true>, pg, th, st, ctx->d, forces, energies);
+    else launch(k_pair_fx<false, 2, false>, pg, th, st, ctx->d, forces, energies);
+    return;
+  }
+  ctx->last_pair_kernel = 6;
+  if (ctx->safe_image) {
+    if (e) launch(k_pair<true, true, true, 2>, pg, th, st, ctx->d, forces, energies);
+    else launch(k_pair<false, true, true, 2>, pg, th, st, ctx->d, forces, energies);
+  } else {
+    if (e) launch(k_pair<true, true, false, 2>, pg, th, st, ctx->d, forces, energies);
+    else launch(k_pair<false, true, false, 2>, pg, th, st, ctx->d, forces, energies);
+  }
+}
 template <bool E, bool P, bool SAFE>
 static void launch_pair_mode(tmd_ctx* ctx, dim3 pg, cudaStream_t st, float* forces, double* energies) {
   if (ctx->pair_mode == 1) launch(k_pair<E, P, SAFE, 1>, pg, PAIR_WARPS * 32, st, ctx->d, forces, energies);
@@ -1008,7 +1299,9 @@ static void launch_pair_fx(tmd_ctx* ctx, dim3 pg, cudaStream_t st, float* forces
 static void launch_pair(tmd_ctx* ctx, dim3 pg, cudaStream_t st, float* forces, double* energies) {
   const bool e = energies != nullptr;
   ctx->last_pair_kernel = 0;
-  if (ctx->d.xf_s) {
+  if (pme_on(ctx)) {
+    launch_pair_ewald(ctx, pg, st, forces, energies);
+  } else if (ctx->d.xf_s) {
     if (e) launch_pair_fx<true>(ctx, pg, st, forces, energies);
     else launch_pair_fx<false>(ctx, pg, st, forces, energies);
   } else if (!ctx->periodic && ctx->fx_packed && ctx->pair_mask != 0 && (ctx->pair_mask & ~(T_LJ | T_ELEC)) == 0 &&
@@ -1104,6 +1397,38 @@ static int enqueue_rebuild_rows(tmd_ctx* ctx, const float* pos, int need_bounds,
   return TMD_OK;
 }
 
+// Particle-mesh Ewald reciprocal chain (pme.cuh) up to phi on the grid: spread, then the 3D DFT as lines along z, y,
+// x (with the influence function), y, z.  Six kernels; k_pme_gather follows once the forces buffer holds the pair forces.
+template <typename T>
+static int enqueue_pme_chain(tmd_ctx* ctx, const T* pos, double* energies, cudaStream_t s) {
+  const PmeArgs& a = priv(ctx).pme;
+  const unsigned R = (unsigned)ctx->nrep;
+  launch(k_pme_spread<T>, atoms_grid(ctx, PME_THREADS), PME_THREADS, s, a, pos);
+  TMD_LAUNCHED(ctx, "k_pme_spread");
+  auto nl = [&](int axis) { return pme_lines_log2<T>(a.K[axis], axis); };
+  auto blocks = [&](int axis) {
+    const long long lines = a.ktot / a.K[axis], per = 1ll << nl(axis);
+    return dim3((unsigned)((lines + per - 1) / per), R);
+  };
+  launch(k_pme_fft<T, PME_FIRST>, blocks(2), PME_THREADS, s, a, 2, nl(2), (double*)nullptr);
+  TMD_LAUNCHED(ctx, "k_pme_fft");
+  launch(k_pme_fft<T, PME_FWD>, blocks(1), PME_THREADS, s, a, 1, nl(1), (double*)nullptr);
+  TMD_LAUNCHED(ctx, "k_pme_fft");
+  launch(k_pme_fft<T, PME_CONV>, blocks(0), PME_THREADS, s, a, 0, nl(0), energies);
+  TMD_LAUNCHED(ctx, "k_pme_fft");
+  launch(k_pme_fft<T, PME_INV>, blocks(1), PME_THREADS, s, a, 1, nl(1), (double*)nullptr);
+  TMD_LAUNCHED(ctx, "k_pme_fft");
+  launch(k_pme_fft<T, PME_INV>, blocks(2), PME_THREADS, s, a, 2, nl(2), (double*)nullptr);
+  TMD_LAUNCHED(ctx, "k_pme_fft");
+  return TMD_OK;
+}
+template <typename T>
+static int enqueue_pme_gather(tmd_ctx* ctx, const T* pos, T* forces, double* energies, cudaStream_t s) {
+  launch(k_pme_gather<T>, atoms_grid(ctx, PME_THREADS), PME_THREADS, s, priv(ctx).pme, pos, forces, energies);
+  TMD_LAUNCHED(ctx, "k_pme_gather");
+  return TMD_OK;
+}
+
 // Forces.compute on an fp64 context: preparation (fp32 shadow), the gated fp32 list build on the shadow, the fp64
 // records in the new order, k_pair_f64, then the two bonded passes in stream order.
 static int enqueue_forces_f64(tmd_ctx* ctx, const double* pos, double* forces, double* energies, cudaStream_t st) {
@@ -1118,13 +1443,18 @@ static int enqueue_forces_f64(tmd_ctx* ctx, const double* pos, double* forces, d
     if (int rc = enqueue_rebuild_rows(ctx, D.shadow, (!ctx->periodic && ctx->cutoff >= 0) ? 1 : 0, st)) return rc;
     launch(k_pack_f64, atoms_grid(ctx, 256), 256, st, d, D, pos);
     TMD_LAUNCHED(ctx, "k_pack_f64");
+    const bool pme = pme_on(ctx);
+    if (pme)
+      if (int rc = enqueue_pme_chain<double>(ctx, pos, energies, st)) return rc;
     CtxPriv& pv = priv(ctx);
     const bool sample = pv.profiling && (size_t)(pv.ev_used + 2) <= pv.ev.size();
     if (sample) TMD_CUDA(cudaEventRecord(pv.ev[pv.ev_used], st));
     const dim3 pg((N + PAIR_WARPS - 1) / PAIR_WARPS, R);
     const int th = PAIR_WARPS * 32;
-    ctx->last_pair_kernel = 5;
-    if (energies && ctx->periodic) launch(k_pair_f64<true, true>, pg, th, st, d, D, forces, energies);
+    ctx->last_pair_kernel = pme ? 8 : 5;
+    if (pme && energies) launch(k_ewpair64<true>, pg, th, st, d, D, forces, energies);
+    else if (pme) launch(k_ewpair64<false>, pg, th, st, d, D, forces, energies);
+    else if (energies && ctx->periodic) launch(k_pair_f64<true, true>, pg, th, st, d, D, forces, energies);
     else if (energies) launch(k_pair_f64<true, false>, pg, th, st, d, D, forces, energies);
     else if (ctx->periodic) launch(k_pair_f64<false, true>, pg, th, st, d, D, forces, energies);
     else launch(k_pair_f64<false, false>, pg, th, st, d, D, forces, energies);
@@ -1133,6 +1463,8 @@ static int enqueue_forces_f64(tmd_ctx* ctx, const double* pos, double* forces, d
       TMD_CUDA(cudaEventRecord(pv.ev[pv.ev_used + 1], st));
       pv.ev_used += 2;
     }
+    if (pme)
+      if (int rc = enqueue_pme_gather<double>(ctx, pos, forces, energies, st)) return rc;
   } else {
     TMD_CUDA(cudaMemsetAsync(forces, 0, (size_t)R * N * 3 * sizeof(double), st));
   }
@@ -1153,6 +1485,16 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
   const int N = ctx->natoms, R = ctx->nrep;
   ctx->force_calls++;
   if (energies) TMD_CUDA(cudaMemsetAsync(energies, 0, (size_t)R * TMD_NUM_ENERGIES * sizeof(double), st));
+  // particle-mesh Ewald: the reciprocal chain needs only the positions, so it runs on its own stream beside the list
+  // check and the pair kernel; k_pme_gather joins it after the pair kernel
+  const bool pme = pme_on(ctx);
+  if (pme) {
+    CtxPriv& pv = priv(ctx);
+    TMD_CUDA(cudaEventRecord(pv.pme_fork, st));
+    TMD_CUDA(cudaStreamWaitEvent(pv.pme_side, pv.pme_fork, 0));
+    if (int prc = enqueue_pme_chain<float>(ctx, pos, energies, pv.pme_side)) return prc;
+    TMD_CUDA(cudaEventRecord(pv.pme_join, pv.pme_side));
+  }
 
   BondedTables T;
   const bool have_bonded = ctx->bonded_nentries > 0;
@@ -1268,7 +1610,13 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
     CtxPriv& pv = priv(ctx);
     const bool sample = pv.profiling && (size_t)(pv.ev_used + 2) <= pv.ev.size();
     if (sample) TMD_CUDA(cudaEventRecord(pv.ev[pv.ev_used], st));
-    if (d.cl.on) {
+    if (d.cl.on && pme) {
+      ctx->last_pair_kernel = 10;
+      const SwitchConsts sc = make_switch_consts_ewald(d.pp);
+      const dim3 cg(pv.cl_blocks, R);
+      if (energies) launch_smem(k_cpair_ew<true>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
+      else launch_smem(k_cpair_ew<false>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
+    } else if (d.cl.on) {
       ctx->last_pair_kernel = 4;
       const SwitchConsts sc = make_switch_consts(d.pp);
       const dim3 cg(pv.cl_blocks, R);
@@ -1284,6 +1632,10 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
     if (sample) {
       TMD_CUDA(cudaEventRecord(pv.ev[pv.ev_used + 1], st));
       pv.ev_used += 2;
+    }
+    if (pme) {
+      TMD_CUDA(cudaStreamWaitEvent(st, pv.pme_join, 0));
+      if (int prc = enqueue_pme_gather<float>(ctx, pos, forces, energies, st)) return prc;
     }
   } else {
     TMD_CUDA(cudaMemsetAsync(forces, 0, (size_t)R * N * 3 * sizeof(float), st));
@@ -1834,7 +2186,7 @@ int tmd_set_force_convention(tmd_ctx* ctx, int exact_gradient) {
   ctx->exact_gradient = exact_gradient ? 1 : 0;
   ctx->d.pp.true_gradient = ctx->exact_gradient;  // uniform kernel parameter: takes effect at the next launch
   ctx->d64.pp.true_gradient = ctx->exact_gradient;
-  ctx->pair_mode = (ctx->pair_mask == (T_LJ | T_ELEC) && ctx->d.pp.has_switch && ctx->d.pp.rfa && !ctx->exact_gradient) ? 1 : 0;
+  ctx->pair_mode = pair_mode_of(ctx);
   return TMD_OK;
 }
 
@@ -1843,6 +2195,7 @@ int tmd_set_owned_atoms(tmd_ctx* ctx, int first_atom, int count) {
     return fail(TMD_ERR_ARG, "tmd_set_owned_atoms: range outside the system");
   if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_owned_atoms: fp64 contexts run the whole system on one GPU");
   if (has_constraints(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_owned_atoms: a context with constraints runs the whole system on one GPU");
+  if (pme_on(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_owned_atoms: a particle-mesh Ewald context runs the whole system on one GPU");
   ctx->d.own_lo = first_atom;
   ctx->d.own_n = count;
   ctx->d.own_all = (first_atom == 0 && count == ctx->natoms) ? 1 : 0;
@@ -1950,6 +2303,7 @@ int tmd_dd_create(tmd_ctx* ctx, int rank, int world, unsigned char* handle_out) 
     return fail(TMD_ERR_ARG, "tmd_dd_create: bad arguments (at most 16 ranks)");
   if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_create: fp64 contexts run the whole system on one GPU");
   if (has_constraints(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_create: a context with constraints runs the whole system on one GPU");
+  if (pme_on(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_create: a particle-mesh Ewald context runs the whole system on one GPU");
   if (ctx->nrep != 1) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_create: decomposed runs take one replica");
   static_assert(sizeof(cudaIpcMemHandle_t) == TMD_IPC_HANDLE_BYTES, "IPC handle size");
   DeviceGuard guard(ctx->device);
@@ -1974,6 +2328,7 @@ int tmd_dd_connect(tmd_ctx* ctx, const unsigned char* handles) {
   if (!ctx || !handles) return fail(TMD_ERR_ARG, "tmd_dd_connect: null pointer");
   if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_connect: fp64 contexts run the whole system on one GPU");
   if (has_constraints(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_connect: a context with constraints runs the whole system on one GPU");
+  if (pme_on(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_connect: a particle-mesh Ewald context runs the whole system on one GPU");
   if (!ctx->dd_base) return fail(TMD_ERR_STATE, "tmd_dd_connect: tmd_dd_create has not been called");
   DeviceGuard guard(ctx->device);
   for (int p = 0; p < ctx->dd_world; ++p) {
@@ -1992,6 +2347,7 @@ int tmd_dd_connect(tmd_ctx* ctx, const unsigned char* handles) {
   if (!ctx) return fail(TMD_ERR_ARG, name ": null context");                                   \
   if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, name ": fp64 contexts run the whole system on one GPU"); \
   if (has_constraints(ctx)) return fail(TMD_ERR_UNSUPPORTED, name ": a context with constraints runs the whole system on one GPU"); \
+  if (pme_on(ctx)) return fail(TMD_ERR_UNSUPPORTED, name ": a particle-mesh Ewald context runs the whole system on one GPU"); \
   if (!ctx->dd_connected) return fail(TMD_ERR_STATE, name ": tmd_dd_create / tmd_dd_connect first"); \
   DeviceGuard guard(ctx->device);
 

@@ -88,6 +88,8 @@ class DecomposedIntegrator:
     def __init__(self, system, forces, timestep, device, gamma=None, T=None, group=None, use_graph=True, exchange=None, constraints=None):
         if constraints is not None:
             raise NotImplementedError("constraints run on one GPU: use Integrator(..., constraints=...)")
+        if getattr(forces, "pme", False):
+            raise NotImplementedError("particle-mesh Ewald runs on one GPU: use Integrator with Forces(..., pme=True)")
         if system.pos.dtype == torch.float64:
             raise NotImplementedError("decomposed runs are fp32 only: run 'precision: double' on one GPU")
         if system.pos.shape[0] != 1:
