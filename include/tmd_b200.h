@@ -318,6 +318,40 @@ int tmd_constrain_f64(tmd_ctx* ctx, double* pos_dev, double* vel_dev, const doub
 int tmd_set_pme(tmd_ctx* ctx, double tolerance);
 int tmd_get_pme(tmd_ctx* ctx, double* alpha, int32_t grid[3]);
 
+/* ---- box changes in stream order, and the molecule move of a barostat (library version >= 104) ----
+ *
+ * tmd_rescale_box[_f64](ctx, box_diag_host, stream) gives every replica the box lengths
+ * box_diag_host (R,3), in stream order: no re-finalisation, no allocation, no synchronisation, and
+ * the captured tmd_md_steps step graphs stay valid.  The cell grids keep their cell counts while the
+ * cells stay at least a list radius / nsub wide and otherwise drop to what the box holds; the next
+ * force call rebuilds the lists.  With PME, alpha and the grid stay as they were (the influence
+ * function and the self + background energy follow the box); a later tmd_set_box[_f64] chooses both
+ * again.  The first rescale of a cluster-path context sets the cluster extent bound of a box 10 %
+ * shorter than the one finalised, which makes the captured steps recapture once.  The call changes
+ * nothing and returns TMD_ERR_UNSUPPORTED when the box cannot take this path: a context not yet
+ * finalised (after a setter, or before its first force call), a box that is not periodic, a
+ * decomposed or peer-to-peer context, a box that breaks the guard-free minimum-image condition the
+ * context was set up with, the cluster lists' extent bound, 2 nsub + 1 cells along an axis, PME's
+ * cutoff <= L/2, or the fp64 limit of 4096 A.  The caller then uses tmd_set_box[_f64].
+ *
+ * tmd_set_molecules(ctx, nmol, ptr, atoms, parent) holds a CSR of molecules: the atoms of molecule
+ * m are atoms[ptr[m] .. ptr[m+1]), every atom exactly once, in breadth-first order of a spanning
+ * tree of its bonds; parent[k] is the atom atoms[k] was reached from (an earlier atom of the same
+ * molecule; the first atom is its own parent).  nmol = 0 clears them.
+ * tmd_scale_molecules[_f64](ctx, pos_dev, scale_dev, stream) moves every molecule of every replica
+ * rigidly with its centroid by the per-axis factors scale_dev (R,3) fp64 device memory, relative to
+ * the box the context holds: unwrapped along its tree, centroid c, each atom to
+ * r + (s - 1) c + n (s L - L), n its image in the molecule's unwrapped frame (csrc/barostat.cuh).
+ * Call it before the tmd_rescale_box[_f64] / tmd_set_box[_f64] to the scaled box.
+ *
+ * tmd_step_captures returns how many step graphs tmd_md_steps has captured so far (-1 for NULL). */
+int tmd_rescale_box(tmd_ctx* ctx, const float* box_diag_host, tmd_stream stream);
+int tmd_rescale_box_f64(tmd_ctx* ctx, const double* box_diag_host, tmd_stream stream);
+int tmd_set_molecules(tmd_ctx* ctx, int nmol, const int32_t* ptr, const int32_t* atoms, const int32_t* parent);
+int tmd_scale_molecules(tmd_ctx* ctx, float* pos_dev, const double* scale_dev, tmd_stream stream);
+int tmd_scale_molecules_f64(tmd_ctx* ctx, double* pos_dev, const double* scale_dev, tmd_stream stream);
+int64_t tmd_step_captures(tmd_ctx* ctx);
+
 /* ---- inspection ------------------------------------------------------------ */
 
 /* The reference's neighbour list for one replica: every non-excluded pair

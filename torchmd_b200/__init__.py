@@ -12,5 +12,6 @@ from .integrator import Integrator, kinetic_energy, kinetic_to_temp, maxwell_bol
 from .parameters import TopologyParameters  # noqa: F401
 from .constraints import Constraints  # noqa: F401
 from .wrapper import Wrapper  # noqa: F401
+from .barostat import MonteCarloBarostat  # noqa: F401
 
 __version__ = "0.1.0"

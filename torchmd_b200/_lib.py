@@ -108,7 +108,15 @@ _SIGNATURES = {
     # particle-mesh Ewald (library version >= 103)
     "tmd_set_pme": (C.c_int, [_P, C.c_double]),
     "tmd_get_pme": (C.c_int, [_P, C.POINTER(C.c_double), C.POINTER(C.c_int32 * 3)]),
+    # box rescale and molecule scaling (library version >= 104)
+    "tmd_rescale_box": (C.c_int, [_P, _P, _P]),
+    "tmd_rescale_box_f64": (C.c_int, [_P, _P, _P]),
+    "tmd_set_molecules": (C.c_int, [_P, C.c_int, _P, _P, _P]),
+    "tmd_scale_molecules": (C.c_int, [_P, _P, _P, _P]),
+    "tmd_scale_molecules_f64": (C.c_int, [_P, _P, _P, _P]),
+    "tmd_step_captures": (C.c_int64, [_P]),
 }
+ERR_UNSUPPORTED = -5
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 
 _lib = None
@@ -125,8 +133,8 @@ def lib():
                 "torchmd_b200 has no CPU or PyTorch fallback."
             )
         handle = C.CDLL(LIB_PATH)
-        if not hasattr(handle, "tmd_set_pme"):
-            raise ImportError(f"{LIB_PATH} predates the particle-mesh Ewald entry points: rebuild it (__graft_entry__.build())")
+        if not hasattr(handle, "tmd_rescale_box"):
+            raise ImportError(f"{LIB_PATH} predates the box-rescale entry points: rebuild it (__graft_entry__.build())")
         for name, (res, args) in _SIGNATURES.items():
             fn = getattr(handle, name)
             fn.restype = res

@@ -339,4 +339,27 @@ __global__ void __launch_bounds__(PME_THREADS) k_pme_gather(PmeArgs a, const T* 
   }
 }
 
+// Influence function of replica blockIdx.y from its box a.L, alpha and the B-spline moduli |b(m)|^2 (mod: K[0] + K[1] +
+// K[2] values, the grid's and not the box's, so uploaded once):
+//   G(m) = exp(-pi^2 m^2 / alpha^2) / (pi V m^2 |b_x|^2 |b_y|^2 |b_z|^2),  G(0) = 0,
+// with m_d = (index, folded to [-K/2, K/2]) / L_d.  Runs at finalisation and on every tmd_rescale_box.
+template <typename T>
+__global__ void __launch_bounds__(PME_THREADS) k_pme_influence(PmeArgs a, const double* __restrict__ mod) {
+  const int r = blockIdx.y;
+  const double L0 = a.L[3 * r], L1 = a.L[3 * r + 1], L2 = a.L[3 * r + 2];
+  const double V = L0 * L1 * L2;
+  T* G = static_cast<T*>(const_cast<void*>(a.infl)) + (size_t)r * a.ktot;
+  for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < a.ktot; idx += (long long)gridDim.x * blockDim.x) {
+    const int z = (int)(idx % a.K[2]);
+    const int y = (int)((idx / a.K[2]) % a.K[1]);
+    const int x = (int)(idx / ((long long)a.K[1] * a.K[2]));
+    const double mx = (x > a.K[0] / 2 ? x - a.K[0] : x) / L0;
+    const double my = (y > a.K[1] / 2 ? y - a.K[1] : y) / L1;
+    const double mz = (z > a.K[2] / 2 ? z - a.K[2] : z) / L2;
+    const double m2 = mx * mx + my * my + mz * mz;
+    const double den = M_PI * V * m2 * mod[x] * mod[a.K[0] + y] * mod[a.K[0] + a.K[1] + z];
+    G[idx] = m2 > 0.0 ? (T)(exp(-M_PI * M_PI * m2 / (a.alpha * a.alpha)) / den) : T(0);
+  }
+}
+
 }  // namespace tmd

@@ -24,6 +24,7 @@
 #include "double.cuh"
 #include "constrain.cuh"
 #include "pme.cuh"
+#include "barostat.cuh"
 
 using namespace tmd;
 
@@ -144,6 +145,24 @@ int device_alloc(T** dst, size_t n) {
   return TMD_OK;
 }
 
+// page-locked host memory, so that a cudaMemcpyAsync from it neither stages nor waits (plain memory in the interpreter)
+static void* stage_alloc(size_t bytes) {
+#if defined(TMD_SIMT_HOST)
+  return malloc(bytes);
+#else
+  void* p = nullptr;
+  return cudaMallocHost(&p, bytes) == cudaSuccess ? p : nullptr;
+#endif
+}
+static void stage_free(void* p) {
+  if (!p) return;
+#if defined(TMD_SIMT_HOST)
+  free(p);
+#else
+  cudaFreeHost(p);
+#endif
+}
+
 
 struct CtxPriv {
   // TMD_B200_OVERLAP=1: bonded kernel on a second stream, concurrent with the pair kernel
@@ -221,6 +240,23 @@ struct CtxPriv {
   void *pme_cgrid = nullptr, *pme_infl = nullptr;
   cudaStream_t pme_side = nullptr;  // fp32: the reciprocal chain runs here, beside the pair kernel
   cudaEvent_t pme_fork = nullptr, pme_join = nullptr;
+  double* pme_mod = nullptr;        // B-spline moduli |b(m)|^2 of the grid, K[0] + K[1] + K[2] (k_pme_influence)
+  double pme_q2 = 0.0, pme_qsum = 0.0;  // sum q^2 and sum q (scaled charges): the self and background energies
+  bool pme_pinned = false;          // tmd_rescale_box keeps alpha and the grid; tmd_set_box / tmd_set_pme choose again
+  int64_t step_captures = 0;        // tmd_step_captures: captures of a tmd_md_steps step graph
+  // tmd_rescale_box: the cell grids of the boxes held (host copy), the choices finalize made that a rescale must keep
+  std::vector<Grid> grids;
+  bool grid_fx = false;             // the grids carry fixed-point units (k_pair_fx, cluster path)
+  bool rescaled = false;            // cl.max_extent has been set to the bound every fast-path box keeps
+  double cl_bound = 0.0;            // that bound (A)
+  double* box_dev = nullptr;        // (R,3) box lengths on the device, for tmd_scale_molecules
+  void* rs_stage = nullptr;         // page-locked staging of the per-box tables a rescale copies
+  size_t rs_stage_bytes = 0;
+  cudaEvent_t rs_done = nullptr;    // recorded after the staging was read
+  // tmd_set_molecules: molecule CSR (barostat.cuh)
+  int mol_n = 0;
+  int *mol_ptr = nullptr, *mol_atoms = nullptr, *mol_parent = nullptr;
+  double* mol_u = nullptr;
 };
 
 }  // namespace
@@ -304,7 +340,7 @@ const char* tmd_last_error(void) { return g_err.c_str(); }
 #if defined(TMD_SIMT_HOST)
 int tmd_version(void) { return -100; }  // host SIMT interpreter build (tests/simt): torchmd_b200/_lib.py refuses it
 #else
-int tmd_version(void) { return 103; }  // 101: the "precision: double" entry points (tmd_set_precision, *_f64); 102: constraints; 103: PME
+int tmd_version(void) { return 104; }  // 101: the "precision: double" entry points (tmd_set_precision, *_f64); 102: constraints; 103: PME; 104: box rescale + molecule scaling
 #endif
 
 int tmd_create(tmd_ctx** out, int device, int natoms, int nreplicas) {
@@ -391,11 +427,14 @@ int tmd_destroy(tmd_ctx* ctx) {
     if (b) cudaFree(b);
   {
     CtxPriv& p = priv(ctx);
-    for (void* b : {(void*)p.pme_q, (void*)p.pme_L, (void*)p.pme_tw, (void*)p.pme_econst, (void*)p.pme_qgrid, p.pme_cgrid, p.pme_infl})
+    for (void* b : {(void*)p.pme_q, (void*)p.pme_L, (void*)p.pme_tw, (void*)p.pme_econst, (void*)p.pme_qgrid, p.pme_cgrid, p.pme_infl,
+                    (void*)p.pme_mod, (void*)p.box_dev, (void*)p.mol_ptr, (void*)p.mol_atoms, (void*)p.mol_parent, (void*)p.mol_u})
       if (b) cudaFree(b);
     if (p.pme_side) cudaStreamDestroy(p.pme_side);
     if (p.pme_fork) cudaEventDestroy(p.pme_fork);
     if (p.pme_join) cudaEventDestroy(p.pme_join);
+    if (p.rs_done) cudaEventDestroy(p.rs_done);
+    stage_free(p.rs_stage);
   }
   delete static_cast<tmd_ctx_full*>(ctx);
   return TMD_OK;
@@ -645,10 +684,12 @@ static int set_box(tmd_ctx* ctx, const T* box_diag) {
     priv(ctx).pme_alpha = alpha;
     for (int d = 0; d < 3; ++d) priv(ctx).pme_K[d] = K[d];
   }
+  priv(ctx).pme_pinned = false;
   ctx->periodic = (nzero == 0);
   ctx->box_host.assign(box_diag, box_diag + ctx->nrep * 3);
   ctx->box64_host.assign(box_diag, box_diag + ctx->nrep * 3);
   if (priv(ctx).con_L) TMD_CUDA(cudaMemcpy(priv(ctx).con_L, ctx->box64_host.data(), ctx->nrep * 3 * sizeof(double), cudaMemcpyHostToDevice));
+  if (priv(ctx).box_dev) TMD_CUDA(cudaMemcpy(priv(ctx).box_dev, ctx->box64_host.data(), ctx->nrep * 3 * sizeof(double), cudaMemcpyHostToDevice));
   ctx->have_box = true;
   ctx->touched = true;
   priv(ctx).dirty = true;
@@ -697,6 +738,7 @@ int tmd_set_pme(tmd_ctx* ctx, double tolerance) {
     for (int d = 0; d < 3; ++d) pv.pme_K[d] = K[d];
   }
   pv.pme_tol = tolerance;
+  pv.pme_pinned = false;
   ctx->touched = true;
   pv.dirty = true;
   return TMD_OK;
@@ -718,7 +760,20 @@ static constexpr double F64_POS_LIMIT = 8192.0;  // A: fp64 contexts flag coordi
 
 // Particle-mesh Ewald tables of the context's boxes: the pair kernels' Ewald constants, twiddles, the influence function
 // G(m) with the B-spline moduli, the self + background energies, and the grids.
-static int pme_finalize(tmd_ctx* ctx) {
+static double pme_econst(double alpha, double q2, double qsum, const double* L) {
+  const double V = L[0] * L[1] * L[2];
+  return -alpha / sqrt(M_PI) * q2 - M_PI * qsum * qsum / (2.0 * V * alpha * alpha);
+}
+template <typename T>
+static void launch_pme_influence(tmd_ctx* ctx, cudaStream_t st) {
+  const CtxPriv& pv = priv(ctx);
+  const long long blocks = std::min<long long>((pv.pme.ktot + PME_THREADS - 1) / PME_THREADS, 4 * (long long)ctx->nsm);
+  launch(k_pme_influence<T>, dim3((unsigned)std::max<long long>(blocks, 1), ctx->nrep), PME_THREADS, st, pv.pme, (const double*)pv.pme_mod);
+}
+
+// A rescaled box (tmd_rescale_box) keeps alpha and the grid the context had (pme_pinned): a re-finalisation on the
+// way (grown lists) keeps them too.  Otherwise both are chosen from the boxes held.
+static int pme_finalize(tmd_ctx* ctx, cudaStream_t stream) {
   CtxPriv& pv = priv(ctx);
   if (!ctx->periodic) return fail(TMD_ERR_UNSUPPORTED, "particle-mesh Ewald needs a periodic box on every replica");
   if (ctx->rfa) return fail(TMD_ERR_UNSUPPORTED, "particle-mesh Ewald and the reaction field exclude each other");
@@ -728,7 +783,12 @@ static int pme_finalize(tmd_ctx* ctx) {
                              "and no atom with itself (the exclusion correction sums each row)");
   double alpha;
   int K[3];
-  if (int rc = pme_choose(ctx, pv.pme_tol, ctx->box64_host.data(), &alpha, K)) return rc;
+  if (pv.pme_pinned) {
+    alpha = pv.pme_alpha;
+    for (int d = 0; d < 3; ++d) K[d] = pv.pme_K[d];
+  } else if (int rc = pme_choose(ctx, pv.pme_tol, ctx->box64_host.data(), &alpha, K)) {
+    return rc;
+  }
   pv.pme_alpha = alpha;
   for (int d = 0; d < 3; ++d) pv.pme_K[d] = K[d];
   const double beta = 2.0 * alpha / sqrt(M_PI);
@@ -782,24 +842,11 @@ static int pme_finalize(tmd_ctx* ctx) {
     for (int m = 0; m < K[d]; ++m)
       if (mod[d][m] < 1e-7) mod[d][m] = 0.5 * (mod[d][(m + K[d] - 1) % K[d]] + mod[d][(m + 1) % K[d]]);
   }
-  std::vector<double> G((size_t)R * ktot), econst(R);
-  for (int r = 0; r < R; ++r) {
-    const double* L = &ctx->box64_host[3 * r];
-    const double V = L[0] * L[1] * L[2];
-    econst[r] = -alpha / sqrt(M_PI) * q2 - M_PI * qsum * qsum / (2.0 * V * alpha * alpha);
-    for (int x = 0; x < K[0]; ++x) {
-      const double mx = (x > K[0] / 2 ? x - K[0] : x) / L[0];
-      for (int y = 0; y < K[1]; ++y) {
-        const double my = (y > K[1] / 2 ? y - K[1] : y) / L[1];
-        for (int z = 0; z < K[2]; ++z) {
-          const double mz = (z > K[2] / 2 ? z - K[2] : z) / L[2];
-          const double m2 = mx * mx + my * my + mz * mz;
-          const size_t idx = (size_t)r * ktot + ((size_t)x * K[1] + y) * K[2] + z;
-          G[idx] = m2 > 0.0 ? exp(-M_PI * M_PI * m2 / (alpha * alpha)) / (M_PI * V * m2 * mod[0][x] * mod[1][y] * mod[2][z]) : 0.0;
-        }
-      }
-    }
-  }
+  std::vector<double> econst(R), mods;
+  for (int r = 0; r < R; ++r) econst[r] = pme_econst(alpha, q2, qsum, &ctx->box64_host[3 * r]);
+  for (int d = 0; d < 3; ++d) mods.insert(mods.end(), mod[d].begin(), mod[d].end());
+  pv.pme_q2 = q2;
+  pv.pme_qsum = qsum;
   for (void* b : {(void*)pv.pme_qgrid, pv.pme_cgrid, pv.pme_infl})
     if (b) cudaFree(b);
   pv.pme_qgrid = nullptr;
@@ -809,14 +856,14 @@ static int pme_finalize(tmd_ctx* ctx) {
   if ((rc = upload(&pv.pme_L, ctx->box64_host.data(), ctx->box64_host.size()))) return rc;
   if ((rc = upload(&pv.pme_tw, tw.data(), tw.size()))) return rc;
   if ((rc = upload(&pv.pme_econst, econst.data(), econst.size()))) return rc;
+  if ((rc = upload(&pv.pme_mod, mods.data(), mods.size()))) return rc;
   if ((rc = device_alloc(&pv.pme_qgrid, (size_t)R * ktot))) return rc;
   TMD_CUDA(cudaMemset(pv.pme_qgrid, 0, (size_t)R * ktot * sizeof(unsigned long long)));
   if (f64) {
-    if ((rc = upload(reinterpret_cast<double**>(&pv.pme_infl), G.data(), G.size()))) return rc;
+    if ((rc = device_alloc(reinterpret_cast<double**>(&pv.pme_infl), (size_t)R * ktot))) return rc;
     if ((rc = device_alloc(reinterpret_cast<Cplx<double>**>(&pv.pme_cgrid), (size_t)R * ktot))) return rc;
   } else {
-    std::vector<float> g32(G.begin(), G.end());
-    if ((rc = upload(reinterpret_cast<float**>(&pv.pme_infl), g32.data(), g32.size()))) return rc;
+    if ((rc = device_alloc(reinterpret_cast<float**>(&pv.pme_infl), (size_t)R * ktot))) return rc;
     if ((rc = device_alloc(reinterpret_cast<Cplx<float>**>(&pv.pme_cgrid), (size_t)R * ktot))) return rc;
     if (!pv.pme_side) {
       TMD_CUDA(cudaStreamCreateWithFlags(&pv.pme_side, cudaStreamNonBlocking));
@@ -845,8 +892,65 @@ static int pme_finalize(tmd_ctx* ctx) {
   a.cl_f = cl.on ? cl.f : nullptr;
   a.cl_inv = cl.on ? cl.inv : nullptr;
   a.cl_stride = (long long)cl.slots + 1;
+  if (f64) launch_pme_influence<double>(ctx, stream);
+  else launch_pme_influence<float>(ctx, stream);
+  TMD_CUDA(cudaGetLastError());  // (set-up work: not counted with the force calls' launches)
   return TMD_OK;
 }
+
+// Cell grid of one replica's box L (list radius rl, ctx->d.nsub cells per radius), and the fixed-point units of the
+// pair kernels when priv(ctx).grid_fx.  keep: the cell counts the replica's grid had, which a rescale keeps while the
+// cells stay at least rl / nsub wide (a growing box only widens them) and otherwise lowers to floor(L nsub / rl) --
+// never above the counts the cell arrays were sized for.  null: chosen from the box.  Returns false when a kept grid
+// would fall below 2 nsub + 1 cells along an axis.
+static bool box_grid(tmd_ctx* ctx, Grid& g, const float* L3, double rl, double margin, const int* keep) {
+  const int nsub = ctx->d.nsub;
+  const bool cells = ctx->periodic && ctx->cutoff >= 0;
+  bool ok = true;
+  memset(&g, 0, sizeof(g));
+  g.periodic = ctx->periodic ? 1 : 0;
+  g.ncells = 1;
+  double lmax = 0.0;
+  for (int k = 0; k < 3; ++k) {
+    const float L = L3[k];
+    g.L[k] = L;
+    g.invL[k] = ctx->periodic ? 1.0f / L : 0.f;
+    g.n[k] = 1;
+    if (cells) {
+      int n = std::min((int)floor((double)L * nsub / rl), 128);
+      if (keep) {
+        if (keep[k] > 1) {
+          n = std::min(n, keep[k]);
+          ok = ok && n >= 2 * nsub + 1;
+        } else {
+          n = 1;
+        }
+      }
+      if (n >= 2 * nsub + 1) {
+        g.n[k] = n;
+        g.reach[k] = nsub;
+        g.inv_w[k] = (float)(n / (double)L);
+      }
+    }
+    g.ncells *= g.n[k];
+    lmax = std::max(lmax, (double)L);
+  }
+  if (priv(ctx).grid_fx) {
+    for (int k = 0; k < 3; ++k) {
+      g.fx_unit[k] = (float)((double)g.L[k] / 4294967296.0);
+      g.fx_inv[k] = 4294967296.0 / (double)g.L[k];
+    }
+    const double rmax = ctx->cutoff + 2.0 * ctx->skin + 2.0 * margin;  // no listed pair is further apart
+    double c0, c1;
+    fx_margin(rmax, lmax, &c0, &c1);
+    g.fx_c0 = (float)(c0 * 1.0000002);  // never round the bound down
+    g.fx_c1 = (float)(c1 * 1.0000002);
+  }
+  return ok;
+}
+
+// list radius margin (A) over cutoff + skin: see finalize
+static double list_margin(const tmd_ctx* ctx) { return 0.004 + (ctx->precision == 64 ? 36.0 / 4096.0 : 0.0); }
 
 static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   if (!ctx->have_atoms) return fail(TMD_ERR_STATE, "tmd_set_atoms has not been called");
@@ -888,7 +992,7 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   // true displacement exceeds its shadow displacement by at most 2 sqrt(3) h, a pair's distance by 4 sqrt(3) h < 7h.
   // With the fp32 slack of the build arithmetic and binning (0.004 A) the radius needs 26h + 7h = 33h more; 36h =
   // 0.0088 A is added.
-  const double margin = 0.004 + (f64 ? 36.0 / 4096.0 : 0.0);  // A
+  const double margin = list_margin(ctx);  // A
   if (f64 && ctx->periodic)
     for (int e = 0; e < R * 3; ++e)
       if (ctx->box_host[e] > 4096.f)
@@ -923,44 +1027,6 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
     d.nsub = use_cluster ? std::max(1, (int)floor(rl / cellw + 0.5)) : 2;
   }
 
-  // cell grid per replica
-  std::vector<Grid> grids(R);
-  long long max_cells = 1;
-  double max_density = 0.0;
-  for (int r = 0; r < R; ++r) {
-    Grid& g = grids[r];
-    memset(&g, 0, sizeof(g));
-    g.periodic = ctx->periodic ? 1 : 0;
-    g.ncells = 1;
-    double vol = 1.0;
-    for (int k = 0; k < 3; ++k) {
-      const float L = ctx->box_host[r * 3 + k];
-      g.L[k] = L;
-      g.invL[k] = ctx->periodic ? 1.0f / L : 0.f;
-      g.n[k] = 1;
-      g.reach[k] = 0;
-      g.origin[k] = 0.f;
-      g.inv_w[k] = 0.f;
-      if (ctx->periodic && has_cut) {
-        int n = (int)floor((double)L * d.nsub / rl);
-        n = std::min(n, 128);
-        if (n >= 2 * d.nsub + 1) {
-          g.n[k] = n;
-          g.reach[k] = d.nsub;
-          g.inv_w[k] = (float)(n / (double)L);
-        }
-      }
-      g.ncells *= g.n[k];
-      vol *= L;
-    }
-    max_cells = std::max<long long>(max_cells, g.ncells);
-    if (ctx->periodic) max_density = std::max(max_density, N / vol);
-  }
-  if (!ctx->periodic && has_cut) max_cells = use_cluster ? 40 * 40 * 40 : 64 * 64 * 64;  // (cluster path: a bucket per cell)
-  d.max_cells = (int)max_cells;
-  // full-row list build: a grid of a few cells is shared out over more CTAs than cells
-  d.build_split = (ctx->periodic && max_cells < ctx->nsm) ? (int)std::min<long long>(64, (ctx->nsm + max_cells - 1) / max_cells) : 1;
-
   // guard-free minimum image is valid iff no listed pair can be further than 0.45 L apart
   ctx->safe_image = false;
   if (ctx->periodic && has_cut) {
@@ -971,36 +1037,33 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   d.check_far = ctx->safe_image ? 1 : 0;
   d.pp.true_gradient = ctx->exact_gradient;
   ctx->pair_mode = pair_mode_of(ctx);
-
   // Fixed-point separations in the pair kernel (k_pair_fx): periodic box with the guard-free
   // image condition (TMD_B200_FX=1 or 2).
+  const int fx = env_switch("TMD_B200_FX", TMD_DEFAULT_FX);
+  ctx->fx_packed = fx == 2;
+  priv(ctx).grid_fx = (((fx == 1 || fx == 2) && ctx->safe_image) || (use_cluster && ctx->periodic)) && ctx->pair_mask && !f64;
+
+  // cell grid per replica
+  std::vector<Grid> grids(R);
+  long long max_cells = 1;
+  double max_density = 0.0;
+  for (int r = 0; r < R; ++r) {
+    Grid& g = grids[r];
+    box_grid(ctx, g, &ctx->box_host[r * 3], rl, margin, nullptr);
+    max_cells = std::max<long long>(max_cells, g.ncells);
+    if (ctx->periodic) max_density = std::max(max_density, N / ((double)g.L[0] * g.L[1] * g.L[2]));
+  }
+  if (!ctx->periodic && has_cut) max_cells = use_cluster ? 40 * 40 * 40 : 64 * 64 * 64;  // (cluster path: a bucket per cell)
+  d.max_cells = (int)max_cells;
+  // full-row list build: a grid of a few cells is shared out over more CTAs than cells
+  d.build_split = (ctx->periodic && max_cells < ctx->nsm) ? (int)std::min<long long>(64, (ctx->nsm + max_cells - 1) / max_cells) : 1;
+
   d.xf_s = nullptr;
-  {
-    const int fx = env_switch("TMD_B200_FX", TMD_DEFAULT_FX);
-    ctx->fx_packed = fx == 2;
-    if ((((fx == 1 || fx == 2) && ctx->safe_image) || (use_cluster && ctx->periodic)) && ctx->pair_mask && !f64) {
-      if (!use_cluster) {
-        const size_t n = (size_t)R * N + R;
-        if ((rc = device_alloc(&ctx->xf_buf, n))) return rc;
-        TMD_CUDA(cudaMemset(ctx->xf_buf, 0, n * sizeof(int4)));
-        d.xf_s = ctx->xf_buf;
-      }
-      const double rmax = ctx->cutoff + 2.0 * ctx->skin + 2.0 * margin;  // no listed pair is further apart
-      for (int r = 0; r < R; ++r) {
-        Grid& g = grids[r];
-        double lmax = 0.0;
-        for (int k = 0; k < 3; ++k) {
-          const double L = (double)g.L[k];
-          g.fx_unit[k] = (float)(L / 4294967296.0);
-          g.fx_inv[k] = 4294967296.0 / L;
-          lmax = std::max(lmax, L);
-        }
-        double c0, c1;
-        fx_margin(rmax, lmax, &c0, &c1);
-        g.fx_c0 = (float)(c0 * 1.0000002);  // never round the bound down
-        g.fx_c1 = (float)(c1 * 1.0000002);
-      }
-    }
+  if (priv(ctx).grid_fx && !use_cluster) {
+    const size_t n = (size_t)R * N + R;
+    if ((rc = device_alloc(&ctx->xf_buf, n))) return rc;
+    TMD_CUDA(cudaMemset(ctx->xf_buf, 0, n * sizeof(int4)));
+    d.xf_s = ctx->xf_buf;
   }
 
   // neighbour row capacity
@@ -1231,7 +1294,11 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
     D.pos_limit = has_cut ? F64_POS_LIMIT : INFINITY;  // without a cutoff every pair is listed: nothing to bound
     D.pp.true_gradient = ctx->exact_gradient;
   }
-  if (pme_on(ctx) && (rc = pme_finalize(ctx))) return rc;
+  if (pme_on(ctx) && (rc = pme_finalize(ctx, stream))) return rc;
+  if (!priv(ctx).box_dev && (rc = device_alloc(&priv(ctx).box_dev, (size_t)R * 3))) return rc;
+  TMD_CUDA(cudaMemcpy(priv(ctx).box_dev, ctx->box64_host.data(), (size_t)R * 3 * sizeof(double), cudaMemcpyHostToDevice));
+  priv(ctx).grids = grids;
+  priv(ctx).rescaled = false;
   priv(ctx).dirty = false;
   return TMD_OK;
 }
@@ -1961,6 +2028,7 @@ int tmd_md_steps(tmd_ctx* ctx, int niter, float* pos, float* vel, float* forces,
         if (rc2) return rc2;
         if (ce != cudaSuccess) return fail(TMD_ERR_CUDA, std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce));
         TMD_CUDA(cudaGraphInstantiate(&pv.exec[k], pv.graph[k], 0));
+        ++pv.step_captures;
         pv.step_launches[k] = ctx->launches - l0 - pv.last_body_launches;  // (the body runs on rebuild steps only: not counted)
         ctx->launches = l0;  // the capture launched nothing; replays are counted below
         ctx->force_calls = f0;
@@ -2295,6 +2363,156 @@ int tmd_constrain(tmd_ctx* ctx, float* pos, float* vel, const float* masses, tmd
 int tmd_constrain_f64(tmd_ctx* ctx, double* pos, double* vel, const double* masses, tmd_stream stream) {
   if (ctx) TMD_PRECISION(ctx, 64, "tmd_constrain_f64")
   return constrain_state(ctx, pos, vel, masses, stream, "tmd_constrain_f64");
+}
+
+// ---- box changes without re-finalising, and the molecule move of the barostat -------------------
+extern "C++" {  // (templates inside the C-linkage block)
+template <typename T>
+static int rescale_box(tmd_ctx* ctx, const T* box_diag, tmd_stream stream, const char* name) {
+  if (!ctx || !box_diag) return fail(TMD_ERR_ARG, std::string(name) + ": bad arguments");
+  CtxPriv& pv = priv(ctx);
+  const int R = ctx->nrep;
+  const std::string who = std::string(name) + ": ";
+  for (int e = 0; e < R * 3; ++e)
+    if (!(box_diag[e] > T(0)) || !((double)box_diag[e] < INFINITY)) return fail(TMD_ERR_ARG, who + "box lengths must be positive and finite");
+  if (ctx->dd_base || !ctx->d.own_all) return fail(TMD_ERR_UNSUPPORTED, who + "decomposed and peer-to-peer runs change the box with tmd_set_box");
+  if (pv.dirty || !ctx->have_box) return fail(TMD_ERR_UNSUPPORTED, who + "the context is not finalised (a setter ran, or no force call yet)");
+  if (!ctx->periodic) return fail(TMD_ERR_UNSUPPORTED, who + "the box is not periodic");
+  const bool f64 = ctx->precision == 64;
+  std::vector<float> b32(box_diag, box_diag + R * 3);
+  std::vector<double> b64(box_diag, box_diag + R * 3);
+  float lmin = INFINITY;
+  for (int e = 0; e < R * 3; ++e) lmin = std::min(lmin, b32[e]);
+  if (f64)
+    for (int e = 0; e < R * 3; ++e)
+      if (b32[e] > 4096.f) return fail(TMD_ERR_UNSUPPORTED, who + "fp64 contexts take box lengths up to 4096 A");
+  const double margin = list_margin(ctx), rl = ctx->cutoff + ctx->skin + margin;
+  if (ctx->safe_image && !((ctx->cutoff + 2.0 * ctx->skin + 2.0 * margin) < 0.45 * (double)lmin))
+    return fail(TMD_ERR_UNSUPPORTED, who + "the box is too small for the guard-free minimum image the context was set up with");
+  double cl_bound = pv.cl_bound;
+  if (ctx->d.cl.on) {
+    // cl.max_extent is held by value in the captured steps: at the first rescale it becomes the bound of a box 10 %
+    // shorter than the one finalised (at least the 8 A the path needs), and every later box must keep it
+    const double limit = 0.5 * (double)lmin - rl - ctx->skin - 0.05;
+    if (!pv.rescaled) {
+      float lmin0 = INFINITY;
+      for (const Grid& g : pv.grids)
+        for (int k = 0; k < 3; ++k) lmin0 = std::min(lmin0, g.L[k]);
+      cl_bound = std::max(8.0, std::min((double)ctx->d.cl.max_extent, 0.5 * 0.9 * (double)lmin0 - rl - ctx->skin - 0.05));
+    }
+    if (limit < cl_bound) return fail(TMD_ERR_UNSUPPORTED, who + "the box is too small for the cluster lists' extent bound");
+  }
+  if (pme_on(ctx))
+    for (int e = 0; e < R * 3; ++e)
+      if (ctx->cutoff > 0.5 * b64[e]) return fail(TMD_ERR_UNSUPPORTED, who + "particle-mesh Ewald needs cutoff <= half of every box length");
+  std::vector<Grid> grids(R);
+  for (int r = 0; r < R; ++r)
+    if (!box_grid(ctx, grids[r], &b32[r * 3], rl, margin, pv.grids[r].n))
+      return fail(TMD_ERR_UNSUPPORTED, who + "the cell grid would fall below 2 nsub + 1 cells along an axis");
+  // accepted: nothing above changed the context
+  DeviceGuard guard(ctx->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (ctx->d.cl.on && !pv.rescaled) ctx->d.cl.max_extent = (float)cl_bound;  // (the one recapture)
+  pv.cl_bound = cl_bound;
+  pv.rescaled = true;
+  pv.pme_pinned = pme_on(ctx);
+  ctx->box_host = b32;
+  ctx->box64_host = b64;
+  pv.grids = grids;
+  // staging: grids | box lengths (fp64) | PME self + background energies
+  const size_t gb = (size_t)R * sizeof(Grid), lb = (size_t)R * 3 * sizeof(double), eb = (size_t)R * sizeof(double);
+  if (pv.rs_stage_bytes < gb + lb + eb) {
+    if (pv.rs_done) TMD_CUDA(cudaEventSynchronize(pv.rs_done));
+    stage_free(pv.rs_stage);
+    pv.rs_stage = stage_alloc(gb + lb + eb);
+    if (!pv.rs_stage) return fail(TMD_ERR_CUDA, who + "page-locked staging allocation failed");
+    pv.rs_stage_bytes = gb + lb + eb;
+  }
+  if (!pv.rs_done) TMD_CUDA(cudaEventCreateWithFlags(&pv.rs_done, cudaEventDisableTiming));
+  TMD_CUDA(cudaEventSynchronize(pv.rs_done));  // the previous rescale's copies have read the staging (done long ago in a run)
+  char* sp = static_cast<char*>(pv.rs_stage);
+  memcpy(sp, grids.data(), gb);
+  memcpy(sp + gb, b64.data(), lb);
+  double* ec = reinterpret_cast<double*>(sp + gb + lb);
+  for (int r = 0; r < R; ++r) ec[r] = pme_on(ctx) ? pme_econst(pv.pme_alpha, pv.pme_q2, pv.pme_qsum, &b64[3 * r]) : 0.0;
+  TMD_CUDA(cudaMemcpyAsync(ctx->d.grid, sp, gb, cudaMemcpyHostToDevice, st));
+  for (double* dst : {pv.box_dev, pv.con_L, ctx->L64, pv.pme_L})
+    if (dst) TMD_CUDA(cudaMemcpyAsync(dst, sp + gb, lb, cudaMemcpyHostToDevice, st));
+  if (pme_on(ctx)) {
+    TMD_CUDA(cudaMemcpyAsync(pv.pme_econst, ec, eb, cudaMemcpyHostToDevice, st));
+    if (f64) launch_pme_influence<double>(ctx, st);
+    else launch_pme_influence<float>(ctx, st);
+    TMD_LAUNCHED(ctx, "k_pme_influence");
+  }
+  TMD_CUDA(cudaEventRecord(pv.rs_done, st));
+  // NaN reference positions: the next force call rebuilds the lists (both pair paths, fp64 included)
+  TMD_CUDA(cudaMemsetAsync(ctx->d.pos_ref, 0xFF, (size_t)R * ctx->natoms * sizeof(float4), st));
+  return TMD_OK;
+}
+
+template <typename T>
+static int scale_molecules(tmd_ctx* ctx, T* pos, const double* scale, tmd_stream stream, const char* name) {
+  if (!ctx || !pos || !scale) return fail(TMD_ERR_ARG, std::string(name) + ": null pointer");
+  CtxPriv& pv = priv(ctx);
+  if (pv.mol_n == 0) return fail(TMD_ERR_STATE, std::string(name) + ": call tmd_set_molecules first");
+  if (!pv.box_dev || !ctx->periodic) return fail(TMD_ERR_STATE, std::string(name) + ": needs a finalised context with a periodic box");
+  DeviceGuard guard(ctx->device);
+  const MolTables m{pv.mol_n, ctx->natoms, pv.mol_ptr, pv.mol_atoms, pv.mol_parent, pv.mol_u};
+  launch(k_scale_molecules<T>, dim3((pv.mol_n + MOL_THREADS - 1) / MOL_THREADS, ctx->nrep), MOL_THREADS, (cudaStream_t)stream, m, pos,
+         scale, (const double*)pv.box_dev);
+  TMD_LAUNCHED(ctx, "k_scale_molecules");
+  return TMD_OK;
+}
+}  // extern "C++"
+
+int tmd_rescale_box(tmd_ctx* ctx, const float* box_diag, tmd_stream stream) {
+  if (ctx) TMD_PRECISION(ctx, 32, "tmd_rescale_box")
+  return rescale_box(ctx, box_diag, stream, "tmd_rescale_box");
+}
+int tmd_rescale_box_f64(tmd_ctx* ctx, const double* box_diag, tmd_stream stream) {
+  if (ctx) TMD_PRECISION(ctx, 64, "tmd_rescale_box_f64")
+  return rescale_box(ctx, box_diag, stream, "tmd_rescale_box_f64");
+}
+int64_t tmd_step_captures(tmd_ctx* ctx) { return ctx ? priv(ctx).step_captures : -1; }
+
+int tmd_set_molecules(tmd_ctx* ctx, int nmol, const int32_t* ptr, const int32_t* atoms, const int32_t* parent) {
+  if (!ctx || nmol < 0 || (nmol > 0 && (!ptr || !atoms || !parent))) return fail(TMD_ERR_ARG, "tmd_set_molecules: bad arguments");
+  const int N = ctx->natoms;
+  if (nmol > 0) {
+    if (ptr[0] != 0 || ptr[nmol] != N) return fail(TMD_ERR_ARG, "tmd_set_molecules: the molecules must hold every atom once");
+    std::vector<int> pos_of(N, -1);
+    for (int m = 0; m < nmol; ++m) {
+      if (ptr[m + 1] <= ptr[m]) return fail(TMD_ERR_ARG, "tmd_set_molecules: empty molecule");
+      for (int k = ptr[m]; k < ptr[m + 1]; ++k) {
+        const int a = atoms[k], p = parent[k];
+        if (a < 0 || a >= N || pos_of[a] >= 0) return fail(TMD_ERR_ARG, "tmd_set_molecules: the molecules must hold every atom once");
+        pos_of[a] = k;
+        const bool root = k == ptr[m];
+        // the parent comes earlier in the same molecule (breadth-first order); the first atom is its own
+        if (root ? p != a : (p < 0 || p >= N || pos_of[p] < ptr[m] || pos_of[p] >= k))
+          return fail(TMD_ERR_ARG, "tmd_set_molecules: parent of atom " + std::to_string(a) + " is not an earlier atom of its molecule");
+      }
+    }
+  }
+  DeviceGuard guard(ctx->device);
+  CtxPriv& pv = priv(ctx);
+  pv.mol_n = 0;
+  if (nmol == 0) return TMD_OK;
+  int rc;
+  if ((rc = upload(&pv.mol_ptr, ptr, (size_t)nmol + 1))) return rc;
+  if ((rc = upload(&pv.mol_atoms, atoms, (size_t)N))) return rc;
+  if ((rc = upload(&pv.mol_parent, parent, (size_t)N))) return rc;
+  if (!pv.mol_u && (rc = device_alloc(&pv.mol_u, (size_t)ctx->nrep * N * 3))) return rc;
+  pv.mol_n = nmol;
+  return TMD_OK;
+}
+int tmd_scale_molecules(tmd_ctx* ctx, float* pos, const double* scale, tmd_stream stream) {
+  if (ctx) TMD_PRECISION(ctx, 32, "tmd_scale_molecules")
+  return scale_molecules(ctx, pos, scale, stream, "tmd_scale_molecules");
+}
+int tmd_scale_molecules_f64(tmd_ctx* ctx, double* pos, const double* scale, tmd_stream stream) {
+  if (ctx) TMD_PRECISION(ctx, 64, "tmd_scale_molecules_f64")
+  return scale_molecules(ctx, pos, scale, stream, "tmd_scale_molecules_f64");
 }
 
 // ---- peer-to-peer position exchange (helpers above, next to priv()) ------------------------

@@ -85,7 +85,10 @@ class DecomposedIntegrator:
     construction ``system.pos`` aliases a padded gather buffer.  Single replica only.
     """
 
-    def __init__(self, system, forces, timestep, device, gamma=None, T=None, group=None, use_graph=True, exchange=None, constraints=None):
+    def __init__(self, system, forces, timestep, device, gamma=None, T=None, group=None, use_graph=True, exchange=None, constraints=None,
+                 barostat=None):
+        if barostat is not None:
+            raise NotImplementedError("the Monte Carlo barostat runs on one GPU: use Integrator(..., barostat=...)")
         if constraints is not None:
             raise NotImplementedError("constraints run on one GPU: use Integrator(..., constraints=...)")
         if getattr(forces, "pme", False):

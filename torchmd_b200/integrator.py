@@ -12,6 +12,11 @@ exactly like the reference does (``tests/test_integrator.py`` mock forces).
 ``constraints`` (a ``torchmd_b200.constraints.Constraints``) makes the step RATTLE: rigid waters and,
 with ``kind="hbonds"``, fixed bonds to hydrogen, which allow 2 fs time steps.  The returned ``T`` then
 counts the constrained degrees of freedom out (``Constraints.ndof``); ``Ekin`` stays sum(m v^2 / 2).
+
+``barostat`` (a ``torchmd_b200.barostat.MonteCarloBarostat``) runs at constant pressure: the steps go in chunks that end
+where the step index reaches a multiple of its ``frequency``, and each such chunk is followed by one Monte Carlo volume
+move per replica, which writes the accepted box into ``systems.box``.  The returned energies describe the state after
+the move.
 """
 import ctypes as C
 
@@ -53,7 +58,7 @@ def kinetic_to_temp(Ekin, natoms):
 
 
 class Integrator:
-    def __init__(self, systems, forces, timestep, device, gamma=None, T=None, batch=None, constraints=None):
+    def __init__(self, systems, forces, timestep, device, gamma=None, T=None, batch=None, constraints=None, barostat=None):
         self.dt = timestep / TIMEFACTOR
         self.systems = systems
         self.forces = forces
@@ -89,6 +94,14 @@ class Integrator:
             if constraints.natoms != len(self.masses):
                 raise ValueError(f"constraints are for {constraints.natoms} atoms, the system has {len(self.masses)}")
             self.ndof = constraints.ndof(batch=batch.cpu().numpy() if batch is not None else None)
+        self.barostat = barostat
+        if barostat is not None:
+            box = systems.box
+            diag = torch.diagonal(box, dim1=1, dim2=2)
+            off = box - torch.diag_embed(diag)
+            if not bool((diag > 0).all()) or bool((off != 0).any()):
+                raise RuntimeError("MonteCarloBarostat needs a periodic orthorhombic box on every replica")
+            barostat._bind(self)
 
     def __del__(self):
         try:
@@ -184,32 +197,43 @@ class Integrator:
                 _lib.check(L.tmd_set_force_convention(ctx, 0))
                 f._exact_gradient = False
             ene = self._out[1]
-            # A neighbour list that outgrows its reserved capacity inside the fused call invalidates the call (the
-            # kernels truncate, the library grows the capacity at the stats() check).  The state is three small
-            # tensors: keep a copy and run the call again from it instead of giving up.
-            saved = (s.pos.clone(), s.vel.clone(), s.forces.clone())
-            for attempt in range(6):
-                _lib.check(
-                    getattr(L, "tmd_md_steps" + sfx)(
-                        ctx, niter, s.pos.data_ptr(), s.vel.data_ptr(), s.forces.data_ptr(), self.masses.data_ptr(),
-                        self.dt, gamma, vcoeff, _lib.ptr(noise), self.seed, 0,
-                        ene.data_ptr(), ke.data_ptr(), stream,
+            bar = self.barostat
+            done = 0
+            while done < niter:
+                # with a barostat the steps run in chunks that end where a move is due
+                n = niter - done if bar is None else min(niter - done, bar.frequency - self._step_index % bar.frequency)
+                chunk_noise = noise[done:done + n] if noise is not None and bar is not None else noise
+                # A neighbour list that outgrows its reserved capacity inside the fused call invalidates the call (the
+                # kernels truncate, the library grows the capacity at the stats() check).  The state is three small
+                # tensors: keep a copy and run the call again from it instead of giving up.
+                saved = (s.pos.clone(), s.vel.clone(), s.forces.clone())
+                for attempt in range(6):
+                    _lib.check(
+                        getattr(L, "tmd_md_steps" + sfx)(
+                            ctx, n, s.pos.data_ptr(), s.vel.data_ptr(), s.forces.data_ptr(), self.masses.data_ptr(),
+                            self.dt, gamma, vcoeff, _lib.ptr(chunk_noise), self.seed, 0,
+                            ene.data_ptr(), ke.data_ptr(), stream,
+                        )
                     )
-                )
-                try:
-                    f.stats()
-                    break
-                except _lib.TmdError as err:
-                    if err.code != _lib.ERR_OVERFLOW:
-                        raise
-                    if attempt == 5:
-                        raise RuntimeError("the neighbour lists kept overflowing during Integrator.step") from err
-                    s.pos.copy_(saved[0])
-                    s.vel.copy_(saved[1])
-                    s.forces.copy_(saved[2])
-                    ctx = self._constrained_ctx()  # (re-finalised with the grown capacity on the next call)
-            self._step_index += niter
-            pot = f._format(ene, None, s.pos.dtype, False, True)
+                    try:
+                        f.stats()
+                        break
+                    except _lib.TmdError as err:
+                        if err.code != _lib.ERR_OVERFLOW:
+                            raise
+                        if attempt == 5:
+                            raise RuntimeError("the neighbour lists kept overflowing during Integrator.step") from err
+                        s.pos.copy_(saved[0])
+                        s.vel.copy_(saved[1])
+                        s.forces.copy_(saved[2])
+                        ctx = self._constrained_ctx()  # (re-finalised with the grown capacity on the next call)
+                self._step_index += n
+                done += n
+                pot = None
+                if bar is not None and self._step_index % bar.frequency == 0:
+                    pot = [float(e) for e in bar.attempt(ctx, ene)]
+            if pot is None:
+                pot = f._format(ene, None, s.pos.dtype, False, True)
         else:
             for it in range(niter):
                 _lib.check(
