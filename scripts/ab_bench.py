@@ -1,7 +1,7 @@
 """A/B timing of library variants in ONE process (one system generation, one torch start-up): for tuning sweeps where
 bench.py's full contract (JSON line, end-to-end loop, CPU baseline, clock sampling) per variant would waste box time.
 
-    python scripts/ab_bench.py --steps 1000 "default" "FX=2|TMD_B200_FX=2" "cull+FX=2|TMD_B200_FX=2|/tmp/var/lib_cull.so"
+    python scripts/ab_bench.py --steps 1000 "default" "FX=2|TMD_B200_FX=2" "other+FX=2|TMD_B200_FX=2|/tmp/var/libtmd_b200.so"
 
 A variant is "label|ENV=VALUE,ENV=VALUE|library path" (the last two optional); the pseudo-variable SKIN=<A> sets the
 Verlet skin of that variant.  Every variant starts from the same

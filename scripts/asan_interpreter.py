@@ -4,7 +4,7 @@
     python scripts/asan_interpreter.py            # builds tests/simt/libtmd_simt_asan.so, re-executes under libasan
 
 Device memory is host memory in that build, so an out-of-bounds index in a kernel (global or shared) is an ASan
-report and a non-zero exit.  Covers the default, fixed-point, packed and no-box pair kernels, the culled list build,
+report and a non-zero exit.  Covers the default, fixed-point, packed and no-box pair kernels, the list build,
 row overflow and regrowth, >32 exclusions, the wrap kernel, fused MD steps, the bonded overlap, the exact-gradient
 convention, owned-atom ranges, the in-process peer-to-peer exchange with three ranks, and (cluster_cases) the cluster
 half-list path.  Takes about half an hour.
@@ -22,7 +22,7 @@ def main():
     import test_simt_kernels as T
     from conftest import load_golden
 
-    L = T.load(T.build_simt("_asan", ["BT_CULL=1", "BT_PAIRED=1", "TMD_SIMT_ASAN=1"]))
+    L = T.load(T.build_simt("_asan", ["TMD_SIMT_ASAN=1"]))
     for name, env, kw in (
         ("chain_amber_periodic", {"TMD_B200_FX": "2"}, {}),
         ("water291_rf_switch", {}, {}),
@@ -40,11 +40,11 @@ def main():
     for n in ("water", "mixed", "nobonds", "zerobox"):
         T.test_wrap_kernel(L, n)
     T.test_fused_md_steps_follow_the_reference_trajectories(L)
-    T.test_row_overflow_grows_the_rows_and_recovers(L, L, "culled")
-    T.test_more_than_32_exclusions_per_atom(L, L, "culled")
+    T.test_row_overflow_grows_the_rows_and_recovers(L)
+    T.test_more_than_32_exclusions_per_atom(L)
     T.test_bonded_overlap_is_bit_identical(L)
     T.test_exact_gradient_convention(L)
-    T.test_owned_atom_range_forces_match_the_full_evaluation(L, L, "packed")
+    T.test_owned_atom_range_forces_match_the_full_evaluation(L, "packed")
     T.test_tiny_systems(L)
     cluster_cases()
     print("asan: no report")

@@ -87,10 +87,9 @@ inline cudaError_t cudaGetDeviceCount(int* n) { *n = 1; return cudaSuccess; }
 inline cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
 inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 inline cudaError_t cudaDeviceSynchronize() { return cudaSuccess; }
-enum cudaDeviceAttr { cudaDevAttrMultiProcessorCount, cudaDevAttrCooperativeLaunch };
+enum cudaDeviceAttr { cudaDevAttrMultiProcessorCount };
 inline cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr a, int) { *v = (a == cudaDevAttrMultiProcessorCount) ? 4 : 0; return cudaSuccess; }
 template <typename F> inline cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int* n, F, int, size_t) { *n = 1; return cudaSuccess; }
-inline cudaError_t cudaLaunchCooperativeKernel(const void*, dim3, dim3, void**, size_t, cudaStream_t) { return cudaErrorNotSupported; }
 enum { cudaStreamNonBlocking = 1, cudaEventDisableTiming = 2 };
 // (a created stream is a distinct non-null handle, as on the device: the library tests handles for "in use")
 inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t* s, unsigned) { static long n = 0; *s = reinterpret_cast<cudaStream_t>(++n); return cudaSuccess; }

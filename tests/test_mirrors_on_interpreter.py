@@ -43,8 +43,8 @@ def hostsim(monkeypatch):
 
 @pytest.fixture
 def hostsim_r2(monkeypatch):
-    """The build with every opt-in path compiled in as the default (packed fixed-point pair kernel, culled two-atom
-    list build, overlapped bonded kernel, fused integrate+prepare and bonded fold)."""
+    """The build with every opt-in path compiled in as the default (packed fixed-point pair kernel, overlapped bonded
+    kernel, fused integrate+prepare and bonded fold)."""
     return _install(monkeypatch, "_r2")
 
 
@@ -340,7 +340,7 @@ def test_bench_reference_arm_reports_what_it_measured(monkeypatch, capsys):
 
 def test_round2_default_configuration_passes_the_gpu_tests(hostsim_r2, capsys):
     """The same GPU test functions with every opt-in path compiled in as the default
-    (culled and paired list build, conditional rebuild node, fixed-point fp32x2 pair kernel, overlapped bonded kernel,
+    (fixed-point fp32x2 pair kernel, overlapped bonded kernel,
     fused prepare, graph replay, cluster path): what `pytest -m gpu`, smoke() and the integrator see."""
     import __graft_entry__ as g
     import test_gpu_forces as G

@@ -23,16 +23,10 @@ CSRC = os.path.join(ROOT, "torchmd_b200", "csrc")
 
 VARIANTS = {  # tag -> defines; every interpreter build the tests use (built together, in parallel, when stale)
     "": [],
-    "_cull": ["BT_CULL=1"],
-    "_paired": ["BT_CULL=1", "BT_PAIRED=1"],
-    "_graph": ["TMD_COND_NODE=1"],  # the device-side switch of the rebuild's conditional node compiled in
     # every opt-in path as the default
-    "_r2": ["BT_CULL=1", "BT_PAIRED=1", "TMD_COND_NODE=1", "TMD_DEFAULT_FX=2", "TMD_DEFAULT_OVERLAP=1", "TMD_DEFAULT_FUSEPREP=1", "TMD_DEFAULT_GRAPH=1", "TMD_DEFAULT_CLUSTER=1"],
-    "_cl": ["TMD_DEFAULT_CLUSTER=1", "TMD_COND_NODE=1", "TMD_DEFAULT_GRAPH=1", "TMD_DEFAULT_FUSEPREP=1", "TMD_DEFAULT_OVERLAP=1"],  # the cluster half-list path (cluster.cuh) over the plain kernels
+    "_r2": ["TMD_DEFAULT_FX=2", "TMD_DEFAULT_OVERLAP=1", "TMD_DEFAULT_FUSEPREP=1", "TMD_DEFAULT_GRAPH=1", "TMD_DEFAULT_CLUSTER=1"],
+    "_cl": ["TMD_DEFAULT_CLUSTER=1", "TMD_DEFAULT_GRAPH=1", "TMD_DEFAULT_FUSEPREP=1", "TMD_DEFAULT_OVERLAP=1"],  # the cluster half-list path (cluster.cuh) over the plain kernels
     "_t2": ["FX_SMALLT_MAX_N=2"],
-    "_fxu4": ["PAIR_FX_UNROLL=4"],
-    "_fx2u2": ["PAIR_FX2_UNROLL=2"],
-    "_fx2pipe": ["PAIR_FX2_PIPE=1"],
 }
 
 
@@ -43,8 +37,7 @@ def _simt_command(out, defines):
     # the interpreter builds start from the plain kernels (every opt-in path off) so that a variant is compared
     # with the same baseline whatever the product's defaults are; a variant's own defines come later and win
     keys = {d.split("=")[0] for d in defines}
-    base = [d for d in ("TMD_DEFAULT_FX=0", "TMD_DEFAULT_OVERLAP=0", "TMD_DEFAULT_FUSEPREP=0", "BT_CULL=0", "BT_PAIRED=0", "TMD_DEFAULT_CLUSTER=0",
-                        "TMD_DEFAULT_GRAPH=0", "TMD_COND_NODE=0")
+    base = [d for d in ("TMD_DEFAULT_FX=0", "TMD_DEFAULT_OVERLAP=0", "TMD_DEFAULT_FUSEPREP=0", "TMD_DEFAULT_CLUSTER=0", "TMD_DEFAULT_GRAPH=0")
             if d.split("=")[0] not in keys]
     return cmd + [f"-D{d}" for d in base + list(defines)] + ["-o", out, os.path.join(SIMT_DIR, "simt_lib.cpp")]
 
@@ -86,12 +79,6 @@ def load(path):
 @pytest.fixture(scope="module")
 def simt():
     return load(build_simt())
-
-
-@pytest.fixture(scope="module", params=["_cull", "_paired"])
-def simt_cull(request):
-    """The list build with chunk culling, one atom or two atoms of a cell per warp pass."""
-    return load(build_simt(request.param, VARIANTS[request.param]))
 
 
 class Ctx:
@@ -227,18 +214,23 @@ def test_packed_kernel_without_a_box(simt, name):
 
 
 @pytest.mark.parametrize("name", ["water291_rf_switch", "argon100_cut", "chain_amber_periodic", "chain_amber_vacuum", "water999_eq", "ala2_nobox_rf"])
-def test_culled_list_build_gives_identical_rows(simt, simt_cull, name):
-    """-DBT_CULL=1: chunk culling, run-wise tile fill and the trimmed chunk loop must leave every neighbour row
-    exactly as it was -- forces (summed in row order) are then bitwise equal, as are the exported pairs."""
+def test_list_build_gives_the_reference_pair_set(simt, name):
+    """Chunk culling, run-wise tile fill and the two-atom chunk loop must leave no pair of the reference out of the
+    rows: the exported pair set equals the reference's, and the forces summed over the rows match the goldens."""
+    from oracle import refmd
+
     g = load_golden(name)
-    a, b = Ctx(simt, g), Ctx(simt_cull, g)
-    Fa, Ea = a.forces()
-    Fb, Eb = b.forces()
-    assert np.array_equal(Fa, Fb)
-    assert a.stats.max_neighbours == b.stats.max_neighbours and not b.stats.overflow
-    assert np.array_equal(a.pairs(), b.pairs())
-    a.close()
-    b.close()
+    c = Ctx(simt, g)
+    F, E = c.forces()
+    check_against_golden(c, F, E)
+    assert not c.stats.overflow
+    if "pairs_f32" in g:
+        ref_pairs = g["pairs_f32"]
+    else:  # no stored pair set: the fp32 oracle's, as oracle_check takes it
+        of32 = refmd.OracleForces(params_from_golden(g, precision=torch.float32), c.terms, **golden_cfg(g))
+        ref_pairs = of32.neighbour_pairs(torch.tensor(c.pos[0]), torch.tensor(g["box"])).numpy().astype(np.int32)
+    assert np.array_equal(c.pairs(), ref_pairs)
+    c.close()
 
 
 def test_bonded_overlap_is_bit_identical(simt):
@@ -247,7 +239,7 @@ def test_bonded_overlap_is_bit_identical(simt):
     Fa, Ea = a.forces()
     Fb, Eb = b.forces()
     assert np.array_equal(Fa, Fb)
-    assert b.stats.kernel_launches == a.stats.kernel_launches + 1  # the overlapped path really ran: k_bonded + k_add_bonded
+    assert b.stats.kernel_launches == a.stats.kernel_launches + 1  # the overlapped path really ran: k_add_bonded
     for k in Ea:
         assert np.allclose(Ea[k], Eb[k], rtol=1e-12, atol=1e-9)
     a.close()
@@ -390,44 +382,38 @@ def test_integrate_and_prepare_in_one_kernel_is_bit_identical(simt, extra):
     b.close()
 
 
-@pytest.fixture(scope="module")
-def simt_graph():
-    return load(build_simt("_graph", VARIANTS["_graph"]))
-
-
 @pytest.mark.parametrize("extra", [{}, {"TMD_B200_OVERLAP": "1", "TMD_B200_FX": "2", "TMD_B200_FUSEPREP": "1"}])
-def test_captured_step_with_conditional_rebuild_replays_the_stream_path(simt_graph, extra):
+def test_captured_step_with_conditional_rebuild_replays_the_stream_path(simt, extra):
     """TMD_B200_GRAPH=1 (the interpreter's record-and-replay model of stream capture, tests/simt/stub): tmd_md_steps
     captures one step twice (with / without energy outputs), the rebuild kernels go into the body of an IF node that
     the preparing kernel switches on, and replaying gives the trajectory of the plain stream path bit for bit -- with
     the rebuild kernels launched only on the steps that rebuild."""
     from torchmd_b200 import _lib
 
-    L = simt_graph
-    g, t, a = md_setup(L, env=dict(extra))
-    _, _, b = md_setup(L, env=dict(extra, TMD_B200_GRAPH="1"))
+    g, t, a = md_setup(simt, env=dict(extra))
+    _, _, b = md_setup(simt, env=dict(extra, TMD_B200_GRAPH="1"))
     gamma = 0.1 / (1000.0 / TIMEFACTOR)
     vcoeff = np.sqrt(2.0 * gamma / a.masses.astype(np.float64) * BOLTZMAN * 300.0 * a.dt).astype(np.float32)
     st = [_lib.Stats(), _lib.Stats()]
     for k, c in enumerate((a, b)):
-        assert L.tmd_get_stats(c.h, C.byref(st[k]), None) == 0
+        assert simt.tmd_get_stats(c.h, C.byref(st[k]), None) == 0
     l0, r0 = [s.kernel_launches for s in st], [s.rebuilds for s in st]
     before = (C.c_longlong * 3)()
-    L.simt_graph_counters(before)  # (the model's counters are per process: other tests replay graphs too)
+    simt.simt_graph_counters(before)  # (the model's counters are per process: other tests replay graphs too)
     total = 0
     for niter in (1, 2, 17):
         for c in (a, b):
-            md_steps(L, c, niter, gamma=gamma, vcoeff=vcoeff, seed=5)
+            md_steps(simt, c, niter, gamma=gamma, vcoeff=vcoeff, seed=5)
         total += niter
         assert np.array_equal(a.posw, b.posw) and np.array_equal(a.vel, b.vel) and np.array_equal(a.F, b.F)
         # (energies are block-wise fp64 atomic sums: equal up to the order of the additions)
         assert np.allclose(a.ene, b.ene, rtol=1e-12, atol=1e-9) and np.allclose(a.ke, b.ke, rtol=1e-12, atol=1e-9)
     for k, c in enumerate((a, b)):
-        assert L.tmd_get_stats(c.h, C.byref(st[k]), None) == 0
+        assert simt.tmd_get_stats(c.h, C.byref(st[k]), None) == 0
     rebuilds = st[0].rebuilds - r0[0]
     assert st[1].rebuilds - r0[1] == rebuilds and 2 <= rebuilds < total
     after = (C.c_longlong * 3)()
-    L.simt_graph_counters(after)
+    simt.simt_graph_counters(after)
     replays, ran, skipped = (after[k] - before[k] for k in range(3))
     assert replays == total and ran + skipped == total  # every step was a replay and met its IF node ...
     assert ran == rebuilds                               # ... whose body ran exactly on the steps that rebuilt
@@ -559,19 +545,18 @@ def test_replicas_are_independent_in_the_packed_kernel(simt):
     c.close()
 
 
-@pytest.mark.parametrize("variant", ["default", "packed", "culled"])
-def test_owned_atom_range_forces_match_the_full_evaluation(simt, simt_cull, variant):
+@pytest.mark.parametrize("variant", ["default", "packed"])
+def test_owned_atom_range_forces_match_the_full_evaluation(simt, variant):
     """Decomposed runs (tmd_set_owned_atoms): rows, forces and bonded terms of an owned sub-range equal the same
-    atoms' values in the full evaluation, bit for bit, in every build / kernel variant."""
-    L = simt_cull if variant == "culled" else simt
+    atoms' values in the full evaluation, bit for bit, in every kernel variant."""
     env = {"TMD_B200_FX": "2"} if variant == "packed" else None
     g = load_golden("chain_amber_periodic")
-    full = Ctx(L, g, env=env)
+    full = Ctx(simt, g, env=env)
     Ff, Ef = full.forces()
-    part = Ctx(L, g, env=env)
+    part = Ctx(simt, g, env=env)
     n = part.natoms
     lo, cnt = n // 3, n // 2
-    part.check(L.tmd_set_owned_atoms(part.h, lo, cnt))
+    part.check(simt.tmd_set_owned_atoms(part.h, lo, cnt))
     Fp, Ep = part.forces()
     assert np.array_equal(Fp[0, lo : lo + cnt], Ff[0, lo : lo + cnt])
     assert 0 < abs(Ep["lj"][0]) < abs(Ef["lj"][0]) * 1.0001 + 1.0
@@ -651,7 +636,7 @@ def test_peer_to_peer_exchange_between_ranks_in_one_process(simt, world):
         c.close()
 
 
-def test_packed_kernel_and_culled_build_on_a_3000_atom_box(simt_cull):
+def test_packed_kernel_and_culled_build_on_a_3000_atom_box(simt):
     """A generated 1000-water box (L = 31 A, 6x6x6 cells, default skin): culled build + packed fixed-point kernel
     against the oracle -- forces, energies and the bit-exact pair set."""
     from oracle import refmd
@@ -679,9 +664,9 @@ def test_packed_kernel_and_culled_build_on_a_3000_atom_box(simt_cull):
             self.f._configure(L, self.h, self.check)
             self.check(L.tmd_set_box(self.h, self.box.ctypes.data))
 
-    c = C2(simt_cull, {"TMD_B200_FX": "2"})
+    c = C2(simt, {"TMD_B200_FX": "2"})
     F, E = c.forces()
-    assert simt_cull.tmd_pair_kernel(c.h) == 2
+    assert simt.tmd_pair_kernel(c.h) == 2
     of = refmd.OracleForces(par64, terms, decision_dtype=torch.float32, **cfg)
     pos_t = torch.tensor(c.pos)
     box_t = torch.diag(torch.tensor(g["box"]))[None]
@@ -719,24 +704,6 @@ def test_packed_kernels_with_the_table_in_global_memory(simt_smalltable, name, k
     F2, _ = c.forces(energies=False)
     check_against_golden(c, F2, {})
     c.close()
-
-
-@pytest.mark.parametrize("tag,define,mode", [("_fxu4", "PAIR_FX_UNROLL=4", "1"), ("_fx2u2", "PAIR_FX2_UNROLL=2", "2"), ("_fx2pipe", "PAIR_FX2_PIPE=1", "2")])
-def test_tuning_variants_of_the_pair_loops(tag, define, mode):
-    """The tuning variants of the pair loops (four entries per lane and iteration, two packed evaluations
-    per iteration, software-pipelined gathers) walk the rows correctly: same results as the plain loops."""
-    L = load(build_simt(tag, [define]))
-    for name, kw in (("chain_amber_periodic", {}), ("water999_eq", {"skin": 0.2})):
-        g = load_golden(name)
-        c = Ctx(L, g, env={"TMD_B200_FX": mode}, **kw)
-        F, E = c.forces()
-        assert L.tmd_pair_kernel(c.h) == int(mode)
-        check_against_golden(c, F, E)
-        F2, _ = c.forces(energies=False)
-        check_against_golden(c, F2, {})
-        if "pairs_f32" in g:
-            assert np.array_equal(c.pairs(), g["pairs_f32"])
-        c.close()
 
 
 # ---- edge cases of the list machinery (synthetic systems against the oracle) -------------------------------
@@ -786,11 +753,9 @@ def oracle_check(c, make, coords, box, terms, cfg, F, tol=1e-4):
     return of32.neighbour_pairs(pos_t[0], torch.tensor(box)).numpy().astype(np.int32)
 
 
-@pytest.mark.parametrize("build", ["default", "culled"])
-def test_row_overflow_grows_the_rows_and_recovers(simt, simt_cull, build):
+def test_row_overflow_grows_the_rows_and_recovers(simt):
     """200 atoms inside a 17 A ball of a 77 A box: the density-based row capacity (64) is far too small; the
     overflow protocol (flag -> TMD_ERR_OVERFLOW -> grown rows -> rebuild) must end in the right answer."""
-    L = simt_cull if build == "culled" else simt
     rng = np.random.default_rng(4)
     pts = []
     while len(pts) < 200:  # min distance 2.2 A inside the ball
@@ -801,7 +766,7 @@ def test_row_overflow_grows_the_rows_and_recovers(simt, simt_cull, build):
     make, coords, box = synthetic(200, coords, [77.0, 77.0, 77.0])
     terms, cfg = ["lj", "electrostatics"], dict(cutoff=9.0, rfa=True, switch_dist=7.5)
     for env in ({}, {"TMD_B200_FX": "2"}):
-        c = SynCtx(L, make, coords, box, terms, env=env, **cfg)
+        c = SynCtx(simt, make, coords, box, terms, env=env, **cfg)
         F, E = c.forces()
         assert c.stats.row_capacity >= c.stats.max_neighbours > 64 and not c.stats.overflow
         # (atoms 2.2 A apart with sigma 3.4: |F| ~ 1000 from ~200 large terms of both signs -- fp32 summation error)
@@ -815,10 +780,8 @@ def test_row_overflow_grows_the_rows_and_recovers(simt, simt_cull, build):
         c.close()
 
 
-@pytest.mark.parametrize("build", ["default", "culled"])
-def test_more_than_32_exclusions_per_atom(simt, simt_cull, build):
+def test_more_than_32_exclusions_per_atom(simt):
     """A hub atom bonded to 40 others (its exclusion list no longer fits one per lane)."""
-    L = simt_cull if build == "culled" else simt
     rng = np.random.default_rng(5)
     n = 120
     coords = rng.uniform(2.0, 22.0, (n, 3))
@@ -830,7 +793,7 @@ def test_more_than_32_exclusions_per_atom(simt, simt_cull, build):
     bonds = [(hub, i) for i in leaves]
     make, coords, box = synthetic(n, coords, [24.0, 24.0, 24.0], bonds=bonds)
     terms, cfg = ["lj", "electrostatics", "bonds"], dict(cutoff=5.0, rfa=True, switch_dist=4.0)
-    c = SynCtx(L, make, coords, box, terms, skin=0.4, **cfg)
+    c = SynCtx(simt, make, coords, box, terms, skin=0.4, **cfg)
     F, E = c.forces()
     ref_pairs = oracle_check(c, make, coords, box, terms, cfg, F, tol=2e-4)
     got = c.pairs()

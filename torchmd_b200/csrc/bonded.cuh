@@ -175,42 +175,6 @@ __device__ __forceinline__ void bonded_energy_reduce(const DeviceState& S, const
   }
 }
 
-__global__ void __launch_bounds__(BONDED_THREADS)
-k_bonded(DeviceState S, BondedTables T, const float* __restrict__ q_scaled, const float* __restrict__ pos,
-         float* __restrict__ forces, double* __restrict__ energies, double* __restrict__ scratch) {
-  const int r = blockIdx.y;
-  const int a = S.own_lo + blockIdx.x * blockDim.x + threadIdx.x;  // owned atoms only
-  const size_t base = (size_t)r * S.natoms;
-  BondedEnergies E;
-  if (a < S.own_lo + S.own_n) {
-    const Vec3d f = bonded_force_on_atom(S, T, q_scaled, pos, r, a, E);
-    if (scratch) {
-      // overlapped with the pair kernel on another stream: the fp64 sums go to a scratch
-      // buffer, k_add_bonded folds them into the forces afterwards (same single rounding)
-      double* o = scratch + (base + a) * 3;
-      o[0] = f.x;
-      o[1] = f.y;
-      o[2] = f.z;
-    } else if (S.cl.on) {
-      // cluster path: the pair forces sit in slot order; this kernel brings them home and adds its own sums
-      const float4 pf = S.cl.f[(size_t)r * (S.cl.slots + 1) + S.cl.inv[base + a]];
-      float* out = forces + (base + a) * 3;
-      out[0] = (float)((double)pf.x + f.x);
-      out[1] = (float)((double)pf.y + f.y);
-      out[2] = (float)((double)pf.z + f.z);
-    } else if (T.atom_ptr[a + 1] > T.atom_ptr[a]) {
-      float* out = forces + (base + a) * 3;
-      out[0] = (float)((double)out[0] + f.x);
-      out[1] = (float)((double)out[1] + f.y);
-      out[2] = (float)((double)out[2] + f.z);
-    }
-  }
-  if (energies) {
-    __shared__ double red[BONDED_THREADS / 32];
-    bonded_energy_reduce(S, T, r, E, energies, red);
-  }
-}
-
 // Pass 1: one thread per term.  Terms none of whose atoms this rank owns are skipped (decomposed runs).
 __global__ void __launch_bounds__(BONDED_THREADS)
 k_bonded_terms(DeviceState S, BondedTables T, TermLayout lay, const float* __restrict__ q_scaled, const float* __restrict__ pos,
@@ -292,7 +256,7 @@ k_bonded_sum(DeviceState S, BondedTables T, TermLayout lay, const double* __rest
   }
 }
 
-// forces += bonded sums of k_bonded's scratch mode (owned atoms), rounded once like the in-place path
+// forces += bonded sums of k_bonded_sum's scratch mode (owned atoms), rounded once like the in-place path
 __global__ void __launch_bounds__(BONDED_THREADS)
 k_add_bonded(int natoms, int lo, int cnt, float* __restrict__ forces, const double* __restrict__ scratch) {
   const int a = lo + blockIdx.x * blockDim.x + threadIdx.x;

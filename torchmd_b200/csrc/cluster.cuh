@@ -49,9 +49,6 @@ constexpr int CL_XCAP = 192;   // excluded-partner entries of one cluster the li
 #define CL_WARPS_N 8
 #endif
 constexpr int CL_WARPS = CL_WARPS_N;
-#ifndef CL_BRANCHFREE
-#define CL_BRANCHFREE 1  // evaluate every packed pair (no per-pair branch): the two pairs of a lane interleave
-#endif
 #ifndef CL_UNROLL
 #define CL_UNROLL 1  // batches per loop iteration
 #endif
@@ -61,9 +58,6 @@ constexpr int CL_WARPS = CL_WARPS_N;
 constexpr int CL_UNROLL_N = CL_UNROLL;
 constexpr int CLB_WARPS = 4;   // list build: warps per CTA
 constexpr int CLB_MAXSEG = 160;
-#ifndef CLB_EXACT
-#define CLB_EXACT 1  // list test against the cluster's atoms (1) or its bounding box (0)
-#endif
 constexpr int CL_SIMT_MAX_ENTRIES = 4096;  // interpreter build (tests/simt): entries per cluster its static buffer holds
 constexpr int CL_SIMT_MAX_TYPES = 64;       // ... and atom types its static table holds
 
@@ -305,7 +299,6 @@ __global__ void __launch_bounds__(CLB_WARPS * 32) k_cbuild(DeviceState S) {
       lo[d] = __shfl_sync(0xffffffffu, lo[d], 0);
       hi[d] = __shfl_sync(0xffffffffu, hi[d], 0);
     }
-#if CLB_EXACT
     float ax[CL], ay[CL], az[CL];
 #pragma unroll
     for (int k = 0; k < CL; ++k) {
@@ -315,7 +308,6 @@ __global__ void __launch_bounds__(CLB_WARPS * 32) k_cbuild(DeviceState S) {
       az[k] = __shfl_sync(0xffffffffu, pw.z, k);
     }
     const float rl2x = rl2 * 1.00001f;  // (rounding of the float test must never drop a pair the skin argument counts on)
-#endif
     if (realmask == 0) {  // (cannot happen: padding only ever completes a cluster)
       if (lane == 0) C.meta[cb + c] = make_int2(0, 0);
       continue;
@@ -512,7 +504,6 @@ __global__ void __launch_bounds__(CLB_WARPS * 32) k_cbuild(DeviceState S) {
         sj = sgm.begin + (idx - sh.pre[w][sg]);
         const float4 p = C.xw[sb + sj];
         const float x = p.x + sgm.sx, y = p.y + sgm.sy, z = p.z + sgm.sz;
-#if CLB_EXACT
         // within the list radius of one of the cluster's atoms (a bounding-box test keeps ~15 % more partners: the
         // corners of the box hold no atom); padding records are 1e30 away, a missing cluster atom is at 1e15
         float d2 = INFINITY;
@@ -522,11 +513,6 @@ __global__ void __launch_bounds__(CLB_WARPS * 32) k_cbuild(DeviceState S) {
           d2 = fminf(d2, fmaf(ux, ux, fmaf(uy, uy, uz * uz)));
         }
         take = d2 < rl2x;
-#else
-        const float ex = fmaxf(fmaxf(lo[0] - x, x - hi[0]), 0.f), ey = fmaxf(fmaxf(lo[1] - y, y - hi[1]), 0.f),
-                    ez = fmaxf(fmaxf(lo[2] - z, z - hi[2]), 0.f);
-        take = ex * ex + ey * ey + ez * ez < rl2;  // (padding records are 1e30 away)
-#endif
         if (sgm.own) {  // own row: the clusters in the next half of the row's cyclic order
           const int cj = (sj - row_s) / CL;
           int dd = cj - ci_row;
@@ -916,28 +902,27 @@ __device__ __forceinline__ void cpair_body(const DeviceState& S, const SwitchCon
           in0 = m0 && s.x <= s_in;
           in1 = m1 && s.y <= s_in;
         }
-        if (CL_BRANCHFREE || in0 || in1) {
-          const ClTab tb = tab[tj * CL_H + p];
-          const F2 nqq = f2_mul(NQI[p], f2(qj));
-          F2 elj, neel;
-          F2 nc = cl_coef2<ENERGY, EW>(sc, s, nqq, tb, elj, neel);
-          nc = f2(in0 ? nc.x : 0.f, in1 ? nc.y : 0.f);  // a select: the other half may hold inf / NaN
-          FX[p] = f2_fma(dx, nc, FX[p]);
-          FY[p] = f2_fma(dy, nc, FY[p]);
-          FZ[p] = f2_fma(dz, nc, FZ[p]);
-          GX = f2_fma(dx, nc, GX);
-          GY = f2_fma(dy, nc, GY);
-          GZ = f2_fma(dz, nc, GZ);
-          if (ENERGY) {
-            F2 e1 = f2(in0 ? elj.x : 0.f, in1 ? elj.y : 0.f), e2 = f2(in0 ? neel.x : 0.f, in1 ? neel.y : 0.f);
-            if (!S.own_all) {
-              const F2 wgt = f2(own_i[2 * p] + own_j, own_i[2 * p + 1] + own_j);
-              e1 = f2_mul(e1, wgt);
-              e2 = f2_mul(e2, wgt);
-            }
-            ELJ = f2_add(ELJ, e1);
-            NEEL = f2_add(NEEL, e2);
+        // every packed pair is evaluated (no per-pair branch), so the two pairs of a lane interleave
+        const ClTab tb = tab[tj * CL_H + p];
+        const F2 nqq = f2_mul(NQI[p], f2(qj));
+        F2 elj, neel;
+        F2 nc = cl_coef2<ENERGY, EW>(sc, s, nqq, tb, elj, neel);
+        nc = f2(in0 ? nc.x : 0.f, in1 ? nc.y : 0.f);  // a select: the other half may hold inf / NaN
+        FX[p] = f2_fma(dx, nc, FX[p]);
+        FY[p] = f2_fma(dy, nc, FY[p]);
+        FZ[p] = f2_fma(dz, nc, FZ[p]);
+        GX = f2_fma(dx, nc, GX);
+        GY = f2_fma(dy, nc, GY);
+        GZ = f2_fma(dz, nc, GZ);
+        if (ENERGY) {
+          F2 e1 = f2(in0 ? elj.x : 0.f, in1 ? elj.y : 0.f), e2 = f2(in0 ? neel.x : 0.f, in1 ? neel.y : 0.f);
+          if (!S.own_all) {
+            const F2 wgt = f2(own_i[2 * p] + own_j, own_i[2 * p + 1] + own_j);
+            e1 = f2_mul(e1, wgt);
+            e2 = f2_mul(e2, wgt);
           }
+          ELJ = f2_add(ELJ, e1);
+          NEEL = f2_add(NEEL, e2);
         }
       }
       const float gx = -(GX.x + GX.y), gy = -(GY.x + GY.y), gz = -(GZ.x + GZ.y);
@@ -1035,7 +1020,7 @@ k_cpair_ew(DeviceState S, SwitchConsts sc, double* __restrict__ energies) {
   cpair_body<ENERGY, true, true>(S, sc, energies);
 }
 
-// forces[i] = pair force of the atom's slot  (systems without bonded terms; otherwise k_bonded adds on the way)
+// forces[i] = pair force of the atom's slot  (systems without bonded terms; otherwise k_bonded_sum adds on the way)
 __global__ void k_cunsort(DeviceState S, float* __restrict__ forces) {
   const int r = blockIdx.y;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;

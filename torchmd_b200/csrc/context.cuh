@@ -176,7 +176,6 @@ struct tmd_ctx {
   bool excl_is_set = true;           // the exclusion CSR lists every pair in both rows, once, and no atom with itself
   bool periodic = false;
   bool safe_image = false;           // guard-free minimum image valid (see min_image_fast)
-  int coop_blocks = 0;               // CTAs per replica of the cooperative rebuild kernel (0: separate kernels)
   int pair_mode = 0;                 // 1: LJ+switch + reaction-field Coulomb specialisation
   int exact_gradient = 0;            // tmd_set_force_convention: switched-LJ force as the true gradient
   int last_pair_kernel = 0;          // tmd_pair_kernel(): 0 float (k_pair), 1 k_pair_fx, 2 k_pair_fx2, 3 k_pair2_open

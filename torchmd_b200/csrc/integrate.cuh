@@ -193,7 +193,7 @@ __device__ __forceinline__ void vv_second_body(int natoms, int lo, int cnt, cons
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
       float f;
-      if (FOLD) {  // k_add_bonded's work (bonded.cuh): the bonded sums of the overlapped k_bonded, rounded once
+      if (FOLD) {  // k_add_bonded's work (bonded.cuh): the bonded sums of the overlapped k_bonded_sum, rounded once
         f = forces_rw[a + d];
         const double sb = scratch[a + d];
         if (sb != 0.0) {

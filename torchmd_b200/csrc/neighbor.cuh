@@ -18,16 +18,12 @@
 //                 shared memory (already shifted by their periodic image) and writes,
 //                 for every atom of the cell, all partners within cutoff+skin that are
 //                 not excluded into one 128-byte-aligned row per atom.
-//   k_rebuild     the five kernels above as the phases of ONE cooperative launch
-//                 (grid-wide barriers in between); opt-in, see tmd_b200.cu.
 //
 // Every rebuild kernel returns immediately unless the replica's rebuild flag is
 // set, so the host can enqueue them unconditionally (no host round trip).  The
 // flag, its parity and every counter live on the device: a captured CUDA graph of
 // one step is replayable.
 #pragma once
-#include <cooperative_groups.h>
-
 #include "context.cuh"
 #include "ptx.cuh"
 
@@ -60,12 +56,6 @@ __device__ __forceinline__ int cell_of_point(const Grid& g, float x, float y, fl
 }
 
 // ---- every call ---------------------------------------------------------------
-// -DTMD_COND_NODE=1 compiles the device-side switch of the rebuild's CUDA-graph conditional node
-// (cudaGraphSetConditional, a driver-resolved builtin: the module then carries an undefined symbol
-// that is bound at load time).
-#ifndef TMD_COND_NODE
-#define TMD_COND_NODE 1
-#endif
 // One atom of the per-call preparation: displacement trigger against the positions of the last
 // rebuild, far-position check, refresh of the sorted records (float and fixed-point), largest
 // |coordinate|.  (x, y, z) is the atom's current position.
@@ -78,10 +68,9 @@ __device__ __forceinline__ void prepare_atom(const DeviceState& S, int r, int i,
   if (!(d2 <= S.trigger2)) {  // also true for NaN (= no list yet)
     if (fl[F_REBUILD0 + parity] == 0) {
       fl[F_REBUILD0 + parity] = 1;
-#if TMD_COND_NODE
       // inside a CUDA graph the rebuild kernels sit in the body of a conditional node: switch it on
+      // (cudaGraphSetConditional is a driver-resolved builtin, bound when the module loads)
       if (S.cond) cudaGraphSetConditional((cudaGraphConditionalHandle)S.cond, 1u);
-#endif
     }
   }
   if (S.check_far) {
@@ -131,8 +120,7 @@ __global__ void k_prepare(DeviceState S, const float* __restrict__ pos) {
 
 // ---- rebuild phases -----------------------------------------------------------------
 // Each phase is a device function over a (bx of nbx blocks) slice of the grid with
-// grid-stride loops, so the same code runs as separate gated kernels or as the phases of
-// the single cooperative kernel k_rebuild (one launch per step instead of five).
+// grid-stride loops; the gated kernels below run one phase each.
 
 // non-periodic bounding box
 __device__ __forceinline__ void phase_bounds(const DeviceState& S, int r, int bx, int nbx,
@@ -316,7 +304,7 @@ __device__ __forceinline__ void phase_sort_pack(const DeviceState& S, int r, int
   }
 }
 
-// separate gated kernels (fallback path / non-cooperative devices)
+// gated kernels: a replica without a pending rebuild returns at once
 #define TMD_GATE                                                                    \
   const int parity = (int)(S.counters[0] & 1ull); /* device-resident: replayable */ \
   if (!S.flags[blockIdx.y * F_COUNT + F_REBUILD0 + parity]) return;
@@ -377,13 +365,10 @@ struct Run {
   float sx, sy, sz;
 };
 
-// BT_CULL=1: every 32-candidate chunk of the tile gets a bounding box; an atom only walks
-// the chunks whose box comes within the list radius (the sweep volume is ~5x the list
-// sphere, so most chunks cannot contribute).  Skipped chunks hold no accepted candidate,
-// so the rows are identical to the unculled build.
-#ifndef BT_CULL
-#define BT_CULL 1
-#endif
+// Every 32-candidate chunk of the tile gets a bounding box; an atom only walks the chunks
+// whose box comes within the list radius (the sweep volume is ~5x the list sphere, so most
+// chunks cannot contribute).  Skipped chunks hold no accepted candidate, so the rows are
+// the same as those of a walk over every chunk.
 constexpr int BT_CHUNKS = BT_TILE / 32;
 static_assert(BT_CHUNKS <= 64, "the per-atom chunk mask is 64 bits");
 
@@ -392,14 +377,11 @@ struct BuildShared {
   Run runs[BT_MAXRUN];
   int roff[BT_MAXRUN + 1];  // exclusive prefix of the run lengths
   int counts[BT_MAXI];
-#if BT_CULL
   float bb[BT_CHUNKS][6];   // per chunk: min x,y,z, max x,y,z over its finite records
   int jr[BT_CHUNKS][2];     // per chunk: smallest / largest sorted atom index among its records
-  float2 pp[BT_WARPS][4];   // BT_PAIRED: per warp, the x / y / z of its two atoms side by side (read back as register pairs)
-#endif
+  float2 pp[BT_WARPS][4];   // per warp, the x / y / z of its two atoms side by side (read back as register pairs)
 };
 
-#if BT_CULL
 // bounding boxes of the staged chunks (one warp per chunk; NaN records are left out: they
 // fail every distance test anyway)
 __device__ __forceinline__ void build_chunk_boxes(BuildShared& sh, int fill) {
@@ -426,165 +408,12 @@ __device__ __forceinline__ void build_chunk_boxes(BuildShared& sh, int fill) {
     }
   }
 }
-#endif
 
-template <bool WRAP>
-__device__ __forceinline__ void build_process_tile(const DeviceState& S, const Grid& g, size_t base,
-                                                   BuildShared& sh, int fill, int b0, int nib, bool w0,
-                                                   bool w1, bool w2) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const unsigned lt = (1u << lane) - 1u;
-#if BT_CULL
-  float rl2 = S.rlist2;
-  int cap = S.row_cap;
-  TMD_PIN_F(rl2);  // keep both in registers: the chunk loop otherwise re-reads them from the constant bank
-  TMD_PIN_R(cap);
-#else
-  const float rl2 = S.rlist2;
-  const int cap = S.row_cap;
-#endif
-  for (int ii = warp; ii < nib; ii += BT_WARPS) {
-    const int k = b0 + ii;
-    if (!S.own_all) {  // decomposed run: rows only for the atoms this rank owns
-      const int io = S.perm[base + k];
-      if (io < S.own_lo || io >= S.own_lo + S.own_n) continue;
-    }
-    const float4 pi = S.xw_s[base + k];
-    // exclusions of this atom as sorted indices, one per lane; [exlo, exhi] bounds them so
-    // that the (rare) chunks which can contain one are the only ones paying for the test
-    int ne = 0, my_excl = -1, exlo = 0x7fffffff, exhi = -1, e0 = 0;
-    if (S.excl_ptr) {
-      const int io = S.perm[base + k];
-      e0 = S.excl_ptr[io];
-      ne = S.excl_ptr[io + 1] - e0;
-      for (int eb = 0; eb < ne; eb += 32) {  // more than 32 exclusions: bounds over all, lanes keep the first 32
-        const int v = (eb + lane < ne) ? S.inv[base + S.excl_idx[e0 + eb + lane]] : -1;
-        if (eb == 0) my_excl = v;
-        if (v >= 0) { exlo = min(exlo, v); exhi = max(exhi, v); }
-      }
-      for (int o = 16; o; o >>= 1) {
-        exlo = min(exlo, __shfl_xor_sync(0xffffffffu, exlo, o));
-        exhi = max(exhi, __shfl_xor_sync(0xffffffffu, exhi, o));
-      }
-    }
-    int* __restrict__ row = S.nbr + (base + k) * (size_t)cap;
-    int count = sh.counts[ii];
-#if BT_CULL
-    unsigned long long row_addr = reinterpret_cast<unsigned long long>(row);
-    TMD_PIN_L(row_addr);  // one 64-bit base; a store address is then base + 4*slot
-    unsigned lt_r = lt, lb_r = 1u << lane;
-    smem_addr tile_lane = smem_address(sh.tile) + 16u * (unsigned)lane;  // this lane's record of chunk 0
-    TMD_PIN_R(lt_r);
-    TMD_PIN_R(lb_r);
-    TMD_PIN_R(tile_lane);
-    // chunks whose bounding box is within the list radius of this atom (lane c tests chunks
-    // c and c+32); a dimension folded per pair (WRAP) cannot be used for culling.  `special`:
-    // chunks whose index range can hold the atom itself or one of its exclusions -- only those
-    // pay for the per-candidate index tests.
-    exlo = min(exlo, k);
-    exhi = max(exhi, k);
-    unsigned mh[2], sp[2];  // chunks 0..31 and 32..63
-    {
-      const int nchunks = (fill + 31) >> 5;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int c = lane + 32 * h;
-        bool v = false;
-        if (c < nchunks) {
-          const float* bb = sh.bb[c];
-          float dx = fmaxf(fmaxf(bb[0] - pi.x, pi.x - bb[3]), 0.f);
-          float dy = fmaxf(fmaxf(bb[1] - pi.y, pi.y - bb[4]), 0.f);
-          float dz = fmaxf(fmaxf(bb[2] - pi.z, pi.z - bb[5]), 0.f);
-          if (WRAP) {
-            if (w0) dx = 0.f;
-            if (w1) dy = 0.f;
-            if (w2) dz = 0.f;
-          }
-          // the per-pair test below rounds differently (differences of the same operands, then
-          // squares): 1e-5 relative slack keeps this one conservative
-          v = (dx * dx + dy * dy + dz * dz) * 0.99999f <= rl2;
-        }
-        mh[h] = __ballot_sync(0xffffffffu, v);
-        sp[h] = __ballot_sync(0xffffffffu, v && sh.jr[c][0] <= exhi && sh.jr[c][1] >= exlo);
-      }
-    }
-#pragma unroll 1
-    for (int h = 0; h < 2; ++h) {
-    unsigned visit = mh[h];
-    const unsigned special = sp[h];
-#pragma unroll 1
-    while (visit) {
-      const int cbit = __ffs((int)visit) - 1;
-      visit &= visit - 1;
-      const float4 pj = lds_f32x4(tile_lane + 512u * (unsigned)(cbit + 32 * h));  // a chunk is 32 records of 16 bytes
-      const bool check_index = (special >> cbit) & 1u;  // warp-uniform
-#else
-    const float4* __restrict__ tp = sh.tile + lane;
-#pragma unroll 1
-    for (int c0 = 0; c0 < fill; c0 += 32, tp += 32) {
-      // candidates beyond `fill` in the last chunk: the tile is padded with far-away records
-      const float4 pj = *tp;
-#endif
-      const int entry = __float_as_int(pj.w);
-      const int j = entry & 0xffffff;
-      float dx = pi.x - pj.x, dy = pi.y - pj.y, dz = pi.z - pj.z;
-      if (WRAP) {  // a dimension too short for cells: one cell spans it, fold per pair
-        if (w0) dx -= g.L[0] * rintf(dx * g.invL[0]);
-        if (w1) dy -= g.L[1] * rintf(dy * g.invL[1]);
-        if (w2) dz -= g.L[2] * rintf(dz * g.invL[2]);
-      }
-#if BT_CULL
-      const bool near = dx * dx + dy * dy + dz * dz <= rl2;
-      unsigned m = __ballot_sync(0xffffffffu, near);
-      if (check_index) {  // rare: the atom itself or an exclusion may be in this chunk
-        bool excl = (j == k);
-#else
-      const bool near = (dx * dx + dy * dy + dz * dz <= rl2) && (j != k);
-      unsigned m = __ballot_sync(0xffffffffu, near);
-      if (__any_sync(0xffffffffu, near && j >= exlo && j <= exhi)) {  // rare: an exclusion may be in this chunk
-        bool excl = false;
-#endif
-        const int nfast = min(ne, 32);
-#pragma unroll 1
-        for (int e = 0; e < nfast; ++e) excl |= (__shfl_sync(0xffffffffu, my_excl, e) == j);
-#pragma unroll 1
-        for (int e = 32; e < ne; ++e) excl |= (S.inv[base + S.excl_idx[e0 + e]] == j);
-        m &= ~__ballot_sync(0xffffffffu, excl);
-      }
-#if BT_CULL
-      const int slot = count + __popc(m & lt_r);
-      if ((m & lb_r) && slot < cap)
-        stg_u32(row_addr + 4ull * (unsigned)slot, entry);
-#else
-      const int slot = count + __popc(m & lt);
-      if (((m >> lane) & 1u) && slot < cap) row[slot] = entry;
-#endif
-      count += __popc(m);
-    }
-#if BT_CULL
-    }  // both halves of the chunk mask
-#endif
-    // keep the row padded to a multiple of 32 entries with the sentinel (record natoms holds
-    // NaN coordinates and fails every cutoff test).  Later tiles overwrite the padding as the
-    // row grows.
-    {
-      const int end = min((count + 31) & ~31, cap);
-      for (int e = count + lane; e < end; e += 32) row[e] = S.natoms;
-    }
-    if (lane == 0) sh.counts[ii] = count;
-  }
-}
-
-// BT_PAIRED=1 (with BT_CULL=1): a warp takes TWO atoms of the cell through the staged chunks at a time.  The
-// candidate record is loaded once for both, the two separations and squared distances are packed fp32x2
-// operations (physics.cuh F2: same rounding per half as the scalar expressions), and a chunk is visited if either
-// atom's bounding-box test asks for it -- a chunk that an atom's own test had culled holds no candidate within its
-// list radius, so visiting it adds nothing to that atom's row.  Rows come out in the same order as in the one-atom
-// loop.  On by default.
-#ifndef BT_PAIRED
-#define BT_PAIRED 1
-#endif
-#if BT_CULL && BT_PAIRED
+// A warp takes TWO atoms of the cell through the staged chunks at a time.  The candidate record is loaded once for
+// both, the two separations and squared distances are packed fp32x2 operations (physics.cuh F2: same rounding per
+// half as the scalar expressions), and a chunk is visited if either atom's bounding-box test asks for it -- a chunk
+// that an atom's own test had culled holds no candidate within its list radius, so visiting it adds nothing to that
+// atom's row.
 struct BuildAtom {
   int k;                        // sorted index
   float4 pi;                    // folded position
@@ -672,6 +501,8 @@ __device__ __forceinline__ void build_process_tile_paired(const DeviceState& S, 
     for (int e = 32; e < a.ne; ++e) excl |= (S.inv[base + S.excl_idx[a.e0 + e]] == j);
     return __ballot_sync(0xffffffffu, excl);
   };
+  // keep the row padded to a multiple of 32 entries with the sentinel (record natoms holds NaN coordinates and fails
+  // every cutoff test).  Later tiles overwrite the padding as the row grows.
   auto finish = [&](const BuildAtom& a, int ii) {
     if (!a.store) return;
     int* row = reinterpret_cast<int*>(a.row_addr);
@@ -757,7 +588,6 @@ __device__ __forceinline__ void build_process_tile_paired(const DeviceState& S, 
     finish(B, i1);
   }
 }
-#endif
 
 __device__ __forceinline__ void phase_build(const DeviceState& S, int r, int bx, int nbx, BuildShared& sh) {
   int* fl = S.flags + r * F_COUNT;
@@ -848,9 +678,8 @@ __device__ __forceinline__ void phase_build(const DeviceState& S, int r, int bx,
       for (int t0 = 0; t0 < M; t0 += BT_TILE) {
         const int fill = min(BT_TILE, M - t0);
         __syncthreads();  // tile free, counts initialised
-#if BT_CULL
-        // one warp per run, lanes stride its records: the same tile layout as the search below
-        // (slot = run offset + position in the run) without a binary search per record
+        // one warp per run, lanes stride its records (tile slot = run offset + position in the run).
+        // The list entry: sorted index (24 bits) + atom type (8 bits), see pair.cuh
         for (int q = tid >> 5; q < BT_MAXRUN; q += BT_WARPS) {
           const Run rn = runs[q];
           const int first = roff[q] - t0;  // tile position of the run's first record (the run may straddle tiles)
@@ -862,35 +691,14 @@ __device__ __forceinline__ void phase_build(const DeviceState& S, int r, int bx,
             tile[at] = make_float4(p.x + rn.sx, p.y + rn.sy, p.z + rn.sz, __int_as_float(j | (S.type_s[base + j] << 24)));
           }
         }
-#else
-        for (int u = tid; u < fill; u += nthr) {
-          const int slot = t0 + u;
-          int q = 0;  // binary search: last run with roff[q] <= slot
-#pragma unroll
-          for (int step = BT_MAXRUN / 2; step; step >>= 1)
-            if (roff[q + step] <= slot) q += step;
-          const Run rn = runs[q];
-          const int j = rn.a0 + (slot - roff[q]);
-          const float4 p = xw[j];
-          // the list entry: sorted index (24 bits) + atom type (8 bits), see pair.cuh
-          tile[u] = make_float4(p.x + rn.sx, p.y + rn.sy, p.z + rn.sz, __int_as_float(j | (S.type_s[base + j] << 24)));
-        }
-#endif
         // pad the last 32-candidate chunk with records that pass no distance test
         for (int u = fill + tid; u < ((fill + 31) & ~31); u += nthr)
           tile[u] = make_float4(NAN, NAN, NAN, __int_as_float(0xffffff));  // NaN: fails `<= rlist2` even when that is +inf
         __syncthreads();
-#if BT_CULL
         build_chunk_boxes(sh, fill);
         __syncthreads();
-#endif
-#if BT_CULL && BT_PAIRED
         if (w0 || w1 || w2) build_process_tile_paired<true>(S, g, base, sh, fill, b0, nib, w0, w1, w2);
         else build_process_tile_paired<false>(S, g, base, sh, fill, b0, nib, w0, w1, w2);
-#else
-        if (w0 || w1 || w2) build_process_tile<true>(S, g, base, sh, fill, b0, nib, w0, w1, w2);
-        else build_process_tile<false>(S, g, base, sh, fill, b0, nib, w0, w1, w2);
-#endif
       }
       __syncthreads();
       for (int t = tid; t < nib; t += nthr) {
@@ -908,42 +716,6 @@ __global__ void __launch_bounds__(BT_WARPS * 32, BT_MINBLOCKS) k_build_list(Devi
   TMD_GATE
   __shared__ BuildShared sh;
   phase_build(S, blockIdx.y, blockIdx.x, gridDim.x, sh);
-}
-
-// The whole rebuild as ONE cooperative launch: phases separated by grid-wide barriers.
-// Enqueued every step; when no replica asked for a rebuild every block returns at once
-// (one ~3 us launch instead of five).  Grid: as many CTAs as are co-resident.
-__global__ void __launch_bounds__(BT_WARPS * 32, BT_MINBLOCKS)
-k_rebuild(DeviceState S, const float* __restrict__ pos, int need_bounds) {
-  const int parity = (int)(S.counters[0] & 1ull);
-  __shared__ int any_s;
-  if (threadIdx.x == 0) {
-    int any = 0;
-    for (int q = 0; q < S.nrep; ++q) any |= S.flags[q * F_COUNT + F_REBUILD0 + parity];
-    any_s = any;
-  }
-  __syncthreads();
-  if (!any_s) return;  // uniform over the grid: nobody reaches a grid barrier
-  cooperative_groups::grid_group grid = cooperative_groups::this_grid();
-  const int r = blockIdx.y, bx = blockIdx.x, nbx = gridDim.x;
-  const bool mine = S.flags[r * F_COUNT + F_REBUILD0 + parity] != 0;
-  __shared__ BuildShared sh;
-  __shared__ int warp_tot[32];
-  if (need_bounds) {
-    if (mine) phase_bounds(S, r, bx, nbx, pos);
-    grid.sync();
-    if (mine && bx == 0 && threadIdx.x == 0) phase_grid(S, r);
-    grid.sync();
-  }
-  if (mine) phase_bin(S, r, bx, nbx, pos);
-  grid.sync();
-  if (mine && bx == 0) phase_scan(S, r, warp_tot);
-  grid.sync();
-  if (mine) phase_place(S, r, bx, nbx);
-  grid.sync();
-  if (mine) phase_sort_pack(S, r, bx, nbx);
-  grid.sync();
-  if (mine) phase_build(S, r, bx, nbx, sh);
 }
 
 // ---- inspection: the reference's neighbour list ----------------------------------------

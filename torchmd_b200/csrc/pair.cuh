@@ -181,9 +181,6 @@ constexpr int FX_PLANE_BYTES = FX_SMALLT_MAX * FX_SMALLT_MAX * 4;  // A plane, t
 #ifndef PAIR_FX_MINBLOCKS
 #define PAIR_FX_MINBLOCKS 5  // 48 registers: at 40 (6 CTAs/SM) ptxas for sm_90a spills inside the neighbour loop
 #endif
-#ifndef PAIR_FX_UNROLL
-#define PAIR_FX_UNROLL 2  // list entries per lane and loop iteration (2 or 4)
-#endif
 
 // Partner record of a replica's fixed-point array at byte offset `off` from `base` (an
 // integer the compiler cannot see through, so the replica's base stays in a register pair
@@ -253,30 +250,6 @@ k_pair_fx(DeviceState S, float* __restrict__ forces, double* __restrict__ energi
       if (s < s_lo) accumulate(entry, wx, wy, wz, s, __int_as_float(pj.w));
       else s_skipped = fminf(s_skipped, s);
     };
-#if PAIR_FX_UNROLL == 4
-    {  // four entries per lane and iteration (tuning variant: two more registers, half the loop overhead)
-      int e = lane;
-      int j0 = (e < n) ? __ldcs(row + e) : -1;
-      int j1 = (e + 32 < n) ? __ldcs(row + e + 32) : -1;
-      int j2 = (e + 64 < n) ? __ldcs(row + e + 64) : -1;
-      int j3 = (e + 96 < n) ? __ldcs(row + e + 96) : -1;
-      while (e < n) {
-        const int jn0 = (e + 128 < n) ? __ldcs(row + e + 128) : -1;
-        const int jn1 = (e + 160 < n) ? __ldcs(row + e + 160) : -1;
-        const int jn2 = (e + 192 < n) ? __ldcs(row + e + 192) : -1;
-        const int jn3 = (e + 224 < n) ? __ldcs(row + e + 224) : -1;
-        if (j0 >= 0) interact(j0, fx_record(xf_base, ((unsigned)j0 << 4) & 0x0ffffff0u));
-        if (j1 >= 0) interact(j1, fx_record(xf_base, ((unsigned)j1 << 4) & 0x0ffffff0u));
-        if (j2 >= 0) interact(j2, fx_record(xf_base, ((unsigned)j2 << 4) & 0x0ffffff0u));
-        if (j3 >= 0) interact(j3, fx_record(xf_base, ((unsigned)j3 << 4) & 0x0ffffff0u));
-        j0 = jn0;
-        j1 = jn1;
-        j2 = jn2;
-        j3 = jn3;
-        e += 128;
-      }
-    }
-#else
     {
       int e = lane;
       int j0 = (e < n) ? __ldcs(row + e) : -1;
@@ -291,7 +264,6 @@ k_pair_fx(DeviceState S, float* __restrict__ forces, double* __restrict__ energi
         e += 64;
       }
     }
-#endif
     if (__any_sync(0xffffffffu, s_skipped <= s_hi)) {
       // rare (a few percent of the rows): re-scan the row and give the pairs inside the band
       // the reference's own decision on the original positions
@@ -340,13 +312,6 @@ k_pair_fx(DeviceState S, float* __restrict__ forces, double* __restrict__ energi
 // partner that is not taken contributes through a zeroed coefficient.
 #ifndef PAIR_FX2_MINBLOCKS
 #define PAIR_FX2_MINBLOCKS 4  // 64 registers: no spills in the loop
-#endif
-#ifndef PAIR_FX2_UNROLL
-#define PAIR_FX2_UNROLL 1  // packed evaluations (pairs of list entries) per lane and loop iteration: 1 or 2
-#endif
-#ifndef PAIR_FX2_PIPE
-#define PAIR_FX2_PIPE 0    // 1: software-pipelined gathers (loads the next records before the current
-                           // pairs are computed, for latency hiding at more registers)
 #endif
 
 // (A_0, A_1), (B_0, B_1) of two partners: from the staged planes (<= 16 types) or from the table in global memory
@@ -444,40 +409,6 @@ __device__ __forceinline__ void pair_fx2_body(const DeviceState& S, const Switch
     }
   };
   auto pair2 = [&](int e0, int j0, int j1) { pair2r(e0, j0, j1, record_of(j0), record_of(j1)); };
-#if PAIR_FX2_PIPE
-  {  // tuning variant: list entries two iterations ahead, partner records one iteration ahead
-    int e = lane;
-    int j0 = entry_at(e), j1 = entry_at(e + 32), jn0 = entry_at(e + 64), jn1 = entry_at(e + 96);
-    int4 p0 = record_of(j0), p1 = record_of(j1);
-    while (e < n) {
-      const int jnn0 = entry_at(e + 128), jnn1 = entry_at(e + 160);
-      const int4 pn0 = record_of(jn0), pn1 = record_of(jn1);
-      pair2r(e, j0, j1, p0, p1);
-      j0 = jn0;
-      j1 = jn1;
-      jn0 = jnn0;
-      jn1 = jnn1;
-      p0 = pn0;
-      p1 = pn1;
-      e += 64;
-    }
-  }
-#elif PAIR_FX2_UNROLL == 2
-  {  // tuning variant: two packed evaluations (four list entries) per iteration
-    int e = lane;
-    int j0 = entry_at(e), j1 = entry_at(e + 32), j2 = entry_at(e + 64), j3 = entry_at(e + 96);
-    while (e < n) {
-      const int jn0 = entry_at(e + 128), jn1 = entry_at(e + 160), jn2 = entry_at(e + 192), jn3 = entry_at(e + 224);
-      pair2(e, j0, j1);
-      pair2(e + 64, j2, j3);
-      j0 = jn0;
-      j1 = jn1;
-      j2 = jn2;
-      j3 = jn3;
-      e += 128;
-    }
-  }
-#else
   {
     int e = lane;
     int j0 = entry_at(e), j1 = entry_at(e + 32);
@@ -489,7 +420,6 @@ __device__ __forceinline__ void pair_fx2_body(const DeviceState& S, const Switch
       e += 64;
     }
   }
-#endif
   float fx = FX.x + FX.y, fy = FY.x + FY.y, fz = FZ.x + FZ.y;
   if (ENERGY) {
     e_lj = ELJ.x + ELJ.y;

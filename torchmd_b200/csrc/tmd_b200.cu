@@ -57,14 +57,8 @@ int fail(int code, const std::string& msg) {
 #ifndef TMD_DEFAULT_FX
 #define TMD_DEFAULT_FX 2        // TMD_B200_FX: 1 fixed-point pair kernel, 2 + fp32x2 arithmetic
 #endif
-#ifndef TMD_DEFAULT_COOP
-#define TMD_DEFAULT_COOP 0      // TMD_B200_COOP: rebuild as one cooperative launch
-#endif
 #ifndef TMD_DEFAULT_OVERLAP
 #define TMD_DEFAULT_OVERLAP 1   // TMD_B200_OVERLAP: bonded kernel on a second stream
-#endif
-#ifndef TMD_DEFAULT_COND
-#define TMD_DEFAULT_COND 0      // TMD_B200_COND: rebuild as a conditional node when captured (needs TMD_COND_NODE)
 #endif
 #ifndef TMD_DEFAULT_GRAPH
 #define TMD_DEFAULT_GRAPH 1     // TMD_B200_GRAPH: tmd_md_steps replays a captured step
@@ -169,13 +163,11 @@ struct CtxPriv {
   cudaStream_t side = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   double* bonded_scratch = nullptr;  // (R,N,3) fp64
-  // TMD_B200_COND=1: when a force call is being captured into a CUDA graph, the rebuild kernels go
-  // into the body of a conditional node that k_prepare switches on (nothing is launched on the
-  // steps that keep their list) instead of five kernels that return at once
-  bool use_cond = false;
-  cudaStream_t helper = nullptr;     // captures the body of the conditional node
-  // TMD_B200_GRAPH=1: tmd_md_steps replays one captured step (two variants: with / without energies)
+  // TMD_B200_GRAPH=1: tmd_md_steps replays one captured step (two variants: with / without energies).  And when a
+  // force call is being captured into a CUDA graph, the rebuild kernels go into the body of a conditional node that
+  // k_prepare switches on (nothing is launched on the steps that keep their list) instead of kernels that return at once
   bool use_graph = false;
+  cudaStream_t helper = nullptr;     // captures the body of the conditional node
   cudaStream_t gstream = nullptr;    // capture + replay stream (the caller's may be the legacy default stream)
   cudaEvent_t ev_in = nullptr, ev_out = nullptr;
   // [0] a whole step, [1] a whole step with the energy outputs (the last, or only, step of a call);
@@ -200,7 +192,6 @@ struct CtxPriv {
   bool fuse_prepare = false;
   double* term_forces = nullptr;  // k_bonded_terms -> k_bonded_sum: force of every (term, slot), fp64 (R x slots x 3)
   size_t term_forces_len = 0;
-  bool bonded_terms = true;       // TMD_B200_BONDED_TERMS=0: the one-kernel atom-centric k_bonded
   bool flags_live = false;  // the device flags hold counts of this context (set by the first finalisation)
   bool fuse_step = false;   // TMD_B200_FUSESTEP=1: k_cstep_boundary between the steps of one tmd_md_steps call
   bool fold_next = false;                       // tmd_md_steps: the vv_second that follows folds the bonded sums in (k_vv_second_fold)
@@ -1021,11 +1012,7 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
     cl_max_extent = 0.5 * (double)lmin - rl - ctx->skin - 0.05;
     use_cluster = cl_max_extent >= cl_extent;
   }
-  {
-    double cellw = 4.0;
-    if (const char* e = getenv("TMD_B200_CELLW")) cellw = std::max(1.0, atof(e));
-    d.nsub = use_cluster ? std::max(1, (int)floor(rl / cellw + 0.5)) : 2;
-  }
+  d.nsub = use_cluster ? std::max(1, (int)floor(rl / 4.0 + 0.5)) : 2;  // cluster path: cells of about 4 A
 
   // guard-free minimum image is valid iff no listed pair can be further than 0.45 L apart
   ctx->safe_image = false;
@@ -1221,28 +1208,13 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
     if ((rc = upload(&ctx->bonded_atom_ptr, ptr.data(), ptr.size()))) return rc;
     if ((rc = upload(&ctx->bonded_entries, ent.data(), ent.size()))) return rc;
     CtxPriv& pv = priv(ctx);
-    pv.bonded_terms = env_switch("TMD_B200_BONDED_TERMS", 1) == 1 || f64;  // (fp64: the two-pass kernels only)
-    const size_t need = pv.bonded_terms ? (size_t)R * ptr[N] * 3 : 0;  // one slot per (term, atom of the term) = per entry
+    const size_t need = (size_t)R * ptr[N] * 3;  // one slot per (term, atom of the term) = per entry
     if (need > pv.term_forces_len) {
       if (pv.term_forces) cudaFree(pv.term_forces);
       pv.term_forces = nullptr;
       pv.term_forces_len = 0;
       if ((rc = device_alloc(&pv.term_forces, need))) return rc;
       pv.term_forces_len = need;
-    }
-  }
-  // cooperative rebuild kernel: as many CTAs as can be co-resident, split over the replicas
-  ctx->coop_blocks = 0;
-  {
-    const bool want_coop = env_switch("TMD_B200_COOP", TMD_DEFAULT_COOP) == 1;
-    int coop = 0, per_sm = 0;
-    cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, ctx->device);
-    // opt-in (TMD_B200_COOP=1): a grid-wide barrier can only deadlock, never fail, if co-residency
-    // is ever violated -- the separate gated kernels are the default
-    if (coop && want_coop &&
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_rebuild, BT_WARPS * 32, 0) == cudaSuccess) {
-      const int total = per_sm * ctx->nsm;
-      if (total >= R) ctx->coop_blocks = std::max(1, total / R);
     }
   }
   // bonded kernel concurrent with the pair kernel (TMD_B200_OVERLAP)
@@ -1264,9 +1236,7 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   {
     CtxPriv& pv = priv(ctx);
     pv.use_graph = env_switch("TMD_B200_GRAPH", TMD_DEFAULT_GRAPH) == 1;
-    // (without the compiled-in node: five gated kernels, as in stream order)
-    pv.use_cond = TMD_COND_NODE && (env_switch("TMD_B200_COND", TMD_DEFAULT_COND) == 1 || pv.use_graph);
-    if (pv.use_cond && !pv.helper) TMD_CUDA(cudaStreamCreateWithFlags(&pv.helper, cudaStreamNonBlocking));
+    if (pv.use_graph && !pv.helper) TMD_CUDA(cudaStreamCreateWithFlags(&pv.helper, cudaStreamNonBlocking));
     if (pv.use_graph && !pv.gstream) {
       TMD_CUDA(cudaStreamCreateWithFlags(&pv.gstream, cudaStreamNonBlocking));
       TMD_CUDA(cudaEventCreateWithFlags(&pv.ev_in, cudaEventDisableTiming));
@@ -1569,11 +1539,6 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
   // bonded forces of the owned atoms: terms in parallel, then the fixed-order sum per atom (bonded.cuh)
   auto launch_bonded = [&](cudaStream_t bs, double* scratch) -> int {
     CtxPriv& pv = priv(ctx);
-    if (!pv.bonded_terms) {
-      launch(k_bonded, owned_grid(ctx, BONDED_THREADS), BONDED_THREADS, bs, d, T, ctx->q, pos, forces, energies, scratch);
-      TMD_LAUNCHED(ctx, "k_bonded");
-      return TMD_OK;
-    }
     const TermLayout lay = term_layout(T);
     launch(k_bonded_terms, dim3((std::max(lay.nterms, 1) + BONDED_THREADS - 1) / BONDED_THREADS, R), BONDED_THREADS, bs, d, T, lay, ctx->q, pos,
            energies, pv.term_forces);
@@ -1597,7 +1562,7 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
     // Being captured into a CUDA graph?  Then the rebuild becomes the body of a conditional node.
     cudaGraph_t cap_graph = nullptr;
     bool in_body = false;
-    if (priv(ctx).use_cond) {
+    if (priv(ctx).use_graph) {
       cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
       if (cudaStreamGetCaptureInfo(st, &cs, nullptr, &cap_graph, nullptr, nullptr) != cudaSuccess ||
           cs != cudaStreamCaptureStatusActive)
@@ -1655,14 +1620,6 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
       TMD_LAUNCHED(ctx, "k_csort");
       launch(k_cbuild, dim3(std::max(1, std::min((d.cl.nclusters_cap + CLB_WARPS - 1) / CLB_WARPS, ctx->nsm * 16)), R), CLB_WARPS * 32, rs, d);
       TMD_LAUNCHED(ctx, "k_cbuild");
-    } else if (ctx->coop_blocks > 0 && !in_body) {
-      // the whole (gated) rebuild in one cooperative launch
-      const float* pos_arg = pos;
-      int nb_arg = need_bounds;
-      void* args[] = {(void*)&d, (void*)&pos_arg, (void*)&nb_arg};
-      TMD_CUDA(cudaLaunchCooperativeKernel((const void*)k_rebuild, dim3(ctx->coop_blocks, R), dim3(BT_WARPS * 32),
-                                           args, 0, st));
-      TMD_LAUNCHED(ctx, "k_rebuild");
     } else {
       if (int brc = enqueue_rebuild_rows(ctx, pos, need_bounds, rs)) return brc;
     }
@@ -1773,7 +1730,7 @@ static int enqueue_constrain_pos_prepare(tmd_ctx* ctx, float* pos, const float* 
   CtxPriv& pv = priv(ctx);
   DeviceState dp = ctx->d;
   pv.prepared_cond = 0;
-  if (pv.use_cond) {
+  if (pv.use_graph) {
     cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
     cudaGraph_t cap_graph = nullptr;
     if (cudaStreamGetCaptureInfo(st, &cs, nullptr, &cap_graph, nullptr, nullptr) == cudaSuccess &&
@@ -1812,7 +1769,7 @@ static int enqueue_vv_first(tmd_ctx* ctx, float* pos, float* vel, const float* f
     // the force call that follows on this stream finds its preparation done
     DeviceState dp = ctx->d;
     pv.prepared_cond = 0;
-    if (pv.use_cond) {
+    if (pv.use_graph) {
       cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
       cudaGraph_t cap_graph = nullptr;
       if (cudaStreamGetCaptureInfo(st, &cs, nullptr, &cap_graph, nullptr, nullptr) == cudaSuccess &&

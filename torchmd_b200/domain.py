@@ -230,8 +230,8 @@ class DecomposedIntegrator:
             try:
                 torch.cuda.synchronize()
                 g = torch.cuda.CUDAGraph()
-                # TMD_B200_COND=1: the library edits the graph under capture (conditional node for the
-                # rebuild kernels, body captured from a helper stream) -- relaxed mode permits that
+                # the library edits the graph under capture (conditional node for the rebuild kernels, body
+                # captured from a helper stream) -- relaxed mode permits that
                 mode = "relaxed"  # (the library turns the rebuild into a conditional node of the graph under capture)
                 with torch.cuda.graph(g, capture_error_mode=mode):
                     self._enqueue_step(with_energy, parity)
