@@ -47,7 +47,7 @@ enum {
 enum {
   TMD_E_BONDS = 0,
   TMD_E_ANGLES = 1,
-  TMD_E_DIHEDRALS = 2,
+  TMD_E_DIHEDRALS = 2, /* proper dihedrals plus the CMAP correction maps (tmd_set_cmap) */
   TMD_E_IMPROPERS = 3,
   TMD_E_14 = 4, /* stays 0: 1-4 energies are booked under lj/electrostatics, forces.py:185-236 */
   TMD_E_ELECTROSTATICS = 5,
@@ -100,6 +100,18 @@ int tmd_set_angles(tmd_ctx* ctx, int n, const int32_t* idx_host, const float* pr
 int tmd_set_torsions(tmd_ctx* ctx, int which, int n, const int32_t* idx_host,
                      const int32_t* term_ptr_host, const float* terms_host, int amber_form);
 int tmd_set_pairs14(tmd_ctx* ctx, int n, const int32_t* idx_host, const float* prm_host);
+
+/* CMAP correction maps (library version >= 105; no reference counterpart).  nmaps grids, map m of
+ * resolution res[m] (4..360), E at (phi_i, psi_j) = grids[off_m + i*res[m] + j], off_m = sum of
+ * res[k]^2 for k < m, phi_i = -180 deg + i * 360 deg / res[m] (psi alike), kcal/mol.  n terms of
+ * 5 atoms, idx (n,5) = (a, b, c, d, e) with phi = dihedral(a,b,c,d), psi = dihedral(b,c,d,e)
+ * (IUPAC sign), map_of (n).  The library builds the spline derivatives and bicubic coefficients
+ * itself (fp64, host, once; CHARMM's construction: periodic cubic splines along each axis, the
+ * cross derivative from a spline along psi of dE/dphi).  Energies are booked in TMD_E_DIHEDRALS;
+ * the terms act when the dihedral bit of the term mask is set.  Either precision (the maps stay
+ * fp64).  n = 0 clears the terms. */
+int tmd_set_cmap(tmd_ctx* ctx, int nmaps, const int32_t* res_host, const double* grids_host,
+                 int n, const int32_t* idx_host, const int32_t* map_of_host);
 
 /* Box diagonal per replica, host (nreplicas,3).  All zeros = no periodic
  * wrapping (forces.py:361).  Sizes the cell grid; call again if the box changes. [sync] */

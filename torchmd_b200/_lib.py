@@ -115,6 +115,8 @@ _SIGNATURES = {
     "tmd_scale_molecules": (C.c_int, [_P, _P, _P, _P]),
     "tmd_scale_molecules_f64": (C.c_int, [_P, _P, _P, _P]),
     "tmd_step_captures": (C.c_int64, [_P]),
+    # CMAP correction maps (library version >= 105)
+    "tmd_set_cmap": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, _P, _P]),
 }
 ERR_UNSUPPORTED = -5
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
@@ -133,8 +135,8 @@ def lib():
                 "torchmd_b200 has no CPU or PyTorch fallback."
             )
         handle = C.CDLL(LIB_PATH)
-        if not hasattr(handle, "tmd_rescale_box"):
-            raise ImportError(f"{LIB_PATH} predates the box-rescale entry points: rebuild it (__graft_entry__.build())")
+        if not hasattr(handle, "tmd_set_cmap"):
+            raise ImportError(f"{LIB_PATH} predates the CMAP entry point: rebuild it (__graft_entry__.build())")
         for name, (res, args) in _SIGNATURES.items():
             fn = getattr(handle, name)
             fn.restype = res

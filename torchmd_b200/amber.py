@@ -18,7 +18,12 @@ semantics step by step:
 * the reference ``Parameters`` builder: unique bonds (i<j), angles (first<last), dihedrals
   (first<last), several terms per dihedral, impropers with the centre in the third slot, 1-4
   pairs = dihedral ends that are not bond/angle exclusions, with scnb / scee from the first
-  term of the dihedral type and Lorentz-Berthelot A/B from the 1-4 LJ values.
+  term of the dihedral type and Lorentz-Berthelot A/B from the 1-4 LJ values;
+* CMAP correction maps (ff19SB, and chamber files with the ``CHARMM_`` prefix), built only
+  when ``amber_parameters`` is asked for ``"cmap"``: ``CMAP_INDEX`` rows are five atoms and a map
+  number, ``CMAP_PARAMETER_nn`` is read phi-major (psi fastest) from -180 deg, the way parmed
+  reads it.  That ordering is restated from format documentation, not pinned against AMBER's
+  own engine.
 
 Pinned by ``tests/test_amber_reader.py`` against the reference's stored known answers for
 ``tests/data/prod_alanine_dipeptide_amber`` (``tests/test_torchmd.py:517,605``,
@@ -27,6 +32,7 @@ Pinned by ``tests/test_amber_reader.py`` against the reference's stored known an
 import math
 import re
 import struct
+import warnings
 from itertools import permutations
 
 import numpy as np
@@ -70,7 +76,7 @@ def read_prmtop(path):
                 flush()
                 flag, fmt, buf = line.split()[1], None, []
             elif line.startswith("%FORMAT"):
-                fmt = line[len("%FORMAT") :].strip().strip("()")
+                fmt = line[len("%FORMAT") :].strip().replace("(", "").replace(")", "")  # also nested: (8(F9.5))
             elif line.startswith("%VERSION") or line.startswith("%COMMENT"):
                 continue
             elif flag is not None:
@@ -129,6 +135,25 @@ class AmberSystem:
         improper = dih[:, 3] < 0
         self.dihedrals = quad[~improper]
         self.impropers = quad[improper]
+
+        # CMAP: terms (a, b, c, d, e) -> map; phi = dihedral(a,b,c,d), psi = dihedral(b,c,d,e)
+        pre = "CHARMM_" if "CHARMM_CMAP_COUNT" in p else ""
+        self.cmap_idx = np.zeros((0, 5), np.int64)
+        self.cmap_map = np.zeros(0, np.int64)
+        self.cmap_res = np.zeros(0, np.int64)
+        self.cmap_grids = []
+        if pre + "CMAP_COUNT" in p:
+            nterm, nmap = p[pre + "CMAP_COUNT"][:2]
+            self.cmap_res = np.array(p[pre + "CMAP_RESOLUTION"][:nmap], dtype=np.int64)
+            for m, r in enumerate(self.cmap_res):
+                g = np.array(p[f"{pre}CMAP_PARAMETER_{m + 1:02d}"], dtype=np.float64)
+                if len(g) != r * r:
+                    raise ValueError(f"{prmtop_path}: CMAP map {m + 1} has {len(g)} values, resolution {r} needs {r * r}")
+                self.cmap_grids.append(g.reshape(r, r))
+            rows = _chunks(p[pre + "CMAP_INDEX"], 6)[:nterm] - 1
+            if len(rows) != nterm or (nterm and (rows[:, 5].min() < 0 or rows[:, 5].max() >= nmap)):
+                raise ValueError(f"{prmtop_path}: CMAP_INDEX does not hold {nterm} terms on maps 1..{nmap}")
+            self.cmap_idx, self.cmap_map = rows[:, :5], rows[:, 5]
 
         # ---- per-type parameters, keyed by AMBER atom-type names like parmed's ParameterSet
         nb_idx = np.array(p["ATOM_TYPE_INDEX"], dtype=np.int64) - 1
@@ -200,7 +225,8 @@ class AmberSystem:
 
 def amber_parameters(system, terms=None, precision=torch.float32, device="cpu"):
     """``TopologyParameters`` for an ``AmberSystem`` -- the reference's
-    ``Parameters(ParmedForcefield(mol, prmtop), mol, terms)`` (parameters.py:109-294)."""
+    ``Parameters(ParmedForcefield(mol, prmtop), mol, terms)`` (parameters.py:109-294).  ``"cmap"`` in ``terms``
+    (not among the defaults) also builds the file's CMAP terms; without it they are left out with a warning."""
     if terms is None:
         terms = ("bonds", "angles", "dihedrals", "impropers", "1-4", "lj")
     terms = [t.lower() for t in terms]
@@ -276,6 +302,13 @@ def amber_parameters(system, terms=None, precision=torch.float32, device="cpu"):
                     rows.append([ep * 4 * s6 * s6, ep * 4 * s6, term[3], term[4]])
                 pmap.append([i, row_of[key]])
             pairs14 = (d14[:, [0, 3]], np.array(pmap, dtype=np.int64), np.array(rows, dtype=np.float64))
+    cmaps = None
+    if len(system.cmap_idx):
+        if "cmap" in terms:
+            cmaps = (system.cmap_idx, system.cmap_map, system.cmap_res, system.cmap_grids)
+        else:
+            warnings.warn(f"the topology has {len(system.cmap_idx)} CMAP terms; they are left out unless terms includes 'cmap'",
+                          stacklevel=2)
     return TopologyParameters(
         atom_types=types,
         type_sigma=sigma,
@@ -287,6 +320,7 @@ def amber_parameters(system, terms=None, precision=torch.float32, device="cpu"):
         dihedrals=dihedrals,
         impropers=impropers,
         pairs14=pairs14,
+        cmaps=cmaps,
         precision=precision,
         device=device,
     )

@@ -13,7 +13,8 @@ _SECTIONS = {"NATOM": 0, "NBOND": 2, "NTHETA": 3, "NPHI": 4, "NIMPHI": 4}
 
 def read_psf(path):
     """dict with atomtype (object array), charge, masses (fp32), bonds (M,2), angles (K,3),
-    dihedrals (D,4), impropers (I,4) as zero-based int64 arrays, plus name/resname/resid/segid."""
+    dihedrals (D,4), impropers (I,4), crossterms (C,8) as zero-based int64 arrays, plus
+    name/resname/resid/segid."""
     with open(path) as fh:
         lines = fh.read().split("\n")
     if not lines or not lines[0].startswith("PSF"):
@@ -62,6 +63,7 @@ def read_psf(path):
         "angles": index_section("NTHETA", 3),
         "dihedrals": index_section("NPHI", 4),
         "impropers": index_section("NIMPHI", 4),
+        "crossterms": index_section("NCRTERM", 8),
     }
 
 
@@ -132,6 +134,8 @@ class CharmmPrmForceField:
     * impropers (harmonic, periodicity 0): parmed keys them by the SORTED type tuple; the adapter tries the
       permutations that keep position 2 (ff_parmed.py:115-129).  This part of parmed is restated from its
       documentation, not pinned: fixtures with impropers are labelled so in tests/golden.
+    * CMAP (not in the reference): a header of the 8 atom types of the two dihedrals and the resolution n, then
+      n * n values, one phi row of n psi values after another from -180 deg; ``get_cmap`` matches the exact 8-tuple.
     """
 
     SECTIONS = ("ATOMS", "BONDS", "ANGLES", "THETAS", "DIHEDRALS", "PHI", "IMPROPER", "IMPROPERS", "IMPHI", "CMAP", "NONBONDED",
@@ -140,6 +144,8 @@ class CharmmPrmForceField:
     def __init__(self, path, mol=None):
         self.mol = mol
         self.bonds, self.angles, self.dihedrals, self.impropers, self.lj, self.masses = {}, {}, {}, {}, {}, {}
+        self.cmaps = {}  # 8 atom types -> (n, n) grid, phi-major
+        cmap_key, cmap_vals, cmap_res = None, [], 0
         section, carry = None, ""
         for raw in open(path):
             line = raw.split("!")[0].strip()
@@ -181,7 +187,20 @@ class CharmmPrmForceField:
                     eps14, rmin14_half = (abs(float(w[5])), float(w[6])) if len(w) >= 7 else (eps, rmin_half)
                     f = 2.0 * 2.0 ** (-1.0 / 6.0)
                     self.lj[t] = (rmin_half * f, eps, rmin14_half * f, eps14)
+                elif section == "CMAP":
+                    if cmap_key is None:  # header: 8 atom types and the resolution
+                        cmap_res = int(w[8])
+                        cmap_key, cmap_vals = tuple(x.upper() for x in w[:8]), []
+                    else:
+                        cmap_vals += [float(x) for x in w]
+                    if len(cmap_vals) >= cmap_res * cmap_res:
+                        if len(cmap_vals) > cmap_res * cmap_res:
+                            raise ValueError(f"{path}: CMAP {cmap_key} holds more than {cmap_res}^2 values")
+                        self.cmaps[cmap_key] = np.array(cmap_vals, dtype=np.float64).reshape(cmap_res, cmap_res)
+                        cmap_key = None
             except (ValueError, IndexError):
+                if section == "CMAP" and cmap_key is not None:
+                    raise ValueError(f"{path}: CMAP {cmap_key} ends after {len(cmap_vals)} of {cmap_res}^2 values") from None
                 continue  # keyword lines inside a section (cutnb ..., HBOND CUTHB ...)
 
     # ---- the reference's _ForceFieldBase interface -------------------------------------------------
@@ -220,6 +239,13 @@ class CharmmPrmForceField:
         self._dihedral_terms((at1, at2, at3, at4))
         l1, l4 = self.lj[str(at1).upper()], self.lj[str(at4).upper()]
         return 1.0, 1.0, l1[2], l1[3], l4[2], l4[3]
+
+    def get_cmap(self, types8):
+        """The (n, n) grid of the cross-term with these 8 atom types (exact match, phi-major, kcal/mol)."""
+        key = tuple(str(a).upper() for a in types8)
+        if key not in self.cmaps:
+            raise RuntimeError(f"Could not find CMAP parameters for {key}")
+        return self.cmaps[key]
 
     def get_improper(self, at1, at2, at3, at4):
         from itertools import permutations

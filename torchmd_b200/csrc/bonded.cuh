@@ -1,9 +1,9 @@
-// bonded.cuh -- bonded terms (K4): bonds, angles, proper/improper torsions, 1-4.
+// bonded.cuh -- bonded terms (K4): bonds, angles, proper/improper torsions, 1-4, CMAP correction maps.
 //
 // Replaces forces.py:122-258 (+ evaluate_bonds/angles/torsion, forces.py:494-605).
 //
 // Two passes, deterministic: k_bonded_terms evaluates every term ONCE (one thread per term, the terms of a kind side by
-// side so that warps do not diverge) and leaves the force on each of its 2-4 atoms in a per-(term, slot) buffer;
+// side so that warps do not diverge) and leaves the force on each of its 2-5 atoms in a per-(term, slot) buffer;
 // k_bonded_sum, one thread per ATOM, walks the list of term instances the atom takes part in (CSR built once on the
 // host from the topology) and adds them up in that fixed order -- no atomics, bitwise reproducible -- then adds the
 // sum to the force array (or hands it to the integrator kernel that folds it in).  A protein's atom sits in ~35 term
@@ -20,12 +20,22 @@ namespace tmd {
 constexpr int BONDED_THREADS = 128;
 
 // kinds of term instance an atom entry can point at
-enum { BK_BOND = 0, BK_ANGLE = 1, BK_DIHEDRAL = 2, BK_IMPROPER = 3, BK_PAIR14 = 4 };
+enum { BK_BOND = 0, BK_ANGLE = 1, BK_DIHEDRAL = 2, BK_IMPROPER = 3, BK_PAIR14 = 4, BK_CMAP = 5 };
+constexpr int BK_KINDS = 6;
+
+// packed atom entry: kind (3 bits) | slot in the term (3 bits) | term index (26 bits)
+__host__ __device__ __forceinline__ unsigned bonded_entry(int kind, int slot, unsigned t) {
+  return ((unsigned)kind << 29) | ((unsigned)slot << 26) | t;
+}
+__device__ __forceinline__ void bonded_unpack(unsigned ent, int& kind, int& slot, int& t) {
+  kind = (int)(ent >> 29), slot = (int)((ent >> 26) & 7u), t = (int)(ent & 0x3ffffffu);
+}
 
 struct BondedTables {
   const int* atom_ptr;   // (natoms+1) CSR over atoms
-  const int* entries;    // packed: kind (3 bits) | slot in the term (2 bits) | term index (27 bits)
+  const int* entries;    // bonded_entry(kind, slot, term)
   BondedSet bonds, angles, torsions[2], pairs14;
+  CmapSet cmap;
 };
 
 struct BoxView {
@@ -51,11 +61,55 @@ struct BondedEnergies {
 // Forces of term t of a kind on each of its atoms (fp64) and its energy; false if the term does not act (a bond
 // beyond the cutoff).  n: atoms of the term.
 struct TermForces {
-  Vec3d f[4];
+  Vec3d f[5];
   double e = 0., e2 = 0.;  // e2: the Coulomb part of a 1-4 pair (e: its LJ part)
-  int atom[4];
+  int atom[5];
   int n = 0;
 };
+
+// CMAP correction map m at (phi, psi) [rad]: bicubic patch of the cell that holds the point (grid from -pi, spacing
+// 2 pi / res, coefficients c[4a+b] of u^a v^b in the cell's unit coordinates).  E, dE/dphi, dE/dpsi; fp64.
+__device__ __forceinline__ double cmap_energy(const CmapSet& C, int m, double phi, double psi, double& dphi, double& dpsi) {
+  const int2 mp = C.maps[m];  // first cell, resolution
+  const int n = mp.y;
+  const double inv_h = (double)n * 0.15915494309189533577;  // n / (2 pi)
+  const double x = (phi + 3.14159265358979323846) * inv_h, y = (psi + 3.14159265358979323846) * inv_h;
+  const double fx = floor(x), fy = floor(y);
+  const double u = x - fx, v = y - fy;
+  int i = (int)fx % n, j = (int)fy % n;
+  if (i < 0) i += n;
+  if (j < 0) j += n;
+  const double* c = C.coef + ((size_t)mp.x + (size_t)i * n + j) * 16;
+  double e = 0., du = 0., dv = 0.;
+#pragma unroll
+  for (int a = 3; a >= 0; --a) {
+    const double r0 = c[4 * a + 0], r1 = c[4 * a + 1], r2 = c[4 * a + 2], r3 = c[4 * a + 3];
+    e = e * u + (((r3 * v + r2) * v + r1) * v + r0);
+    dv = dv * u + ((3.0 * r3 * v + 2.0 * r2) * v + r1);
+  }
+#pragma unroll
+  for (int b = 3; b >= 0; --b) du = du * v + ((3.0 * c[12 + b] * u + 2.0 * c[8 + b]) * u + c[4 + b]);
+  dphi = du * inv_h;
+  dpsi = dv * inv_h;
+  return e;
+}
+
+// A CMAP term (a, b, c, d, e) from its four bond vectors r_k = x_k - x_(k+1): phi = dihedral(a, b, c, d),
+// psi = dihedral(b, c, d, e), the two torsion force projections summed onto the five atoms.
+__device__ __forceinline__ double cmap_term(const CmapSet& C, int t, const Vec3d& r01, const Vec3d& r12, const Vec3d& r23,
+                                           const Vec3d& r34, Vec3d* f) {
+  const TorsionGeom<double> g1 = torsion_geom(r01, r12, r23), g2 = torsion_geom(r12, r23, r34);
+  double dphi, dpsi;
+  const double e = cmap_energy(C, C.map_of[t], g1.phi, g2.phi, dphi, dpsi);
+  Vec3d q0, q1, q2, q3;
+  torsion_forces(g1, dphi, f[0], f[1], f[2], f[3]);
+  torsion_forces(g2, dpsi, q0, q1, q2, q3);
+  f[1] = f[1] + q0;
+  f[2] = f[2] + q1;
+  f[3] = f[3] + q2;
+  f[4] = q3;
+  return e;
+}
 
 __device__ __forceinline__ bool bonded_term(const DeviceState& S, const BondedTables& T, const float* __restrict__ q_scaled,
                                             const float* __restrict__ pos, size_t base, const BoxView& bx, int kind, int t, TermForces& o) {
@@ -102,6 +156,16 @@ __device__ __forceinline__ bool bonded_term(const DeviceState& S, const BondedTa
     o.e = e;
     return true;
   }
+  if (kind == BK_CMAP) {
+    o.n = 5;
+#pragma unroll
+    for (int k = 0; k < 5; ++k) o.atom[k] = T.cmap.idx[5 * t + k];
+    const Vec3 p0 = load3(pos, base + o.atom[0]), p1 = load3(pos, base + o.atom[1]), p2 = load3(pos, base + o.atom[2]);
+    const Vec3 p3 = load3(pos, base + o.atom[3]), p4 = load3(pos, base + o.atom[4]);
+    o.e = cmap_term(T.cmap, t, delta_f64(p0, p1, bx.periodic, bx.L), delta_f64(p1, p2, bx.periodic, bx.L),
+                    delta_f64(p2, p3, bx.periodic, bx.L), delta_f64(p3, p4, bx.periodic, bx.L), o.f);
+    return true;
+  }
   // BK_PAIR14 (forces.py:185-236): LJ/scnb with no cutoff or switch, Coulomb/scee, never RF
   const int i = T.pairs14.idx[2 * t], j = T.pairs14.idx[2 * t + 1];
   o.n = 2, o.atom[0] = i, o.atom[1] = j;
@@ -130,7 +194,7 @@ __device__ __forceinline__ bool bonded_term(const DeviceState& S, const BondedTa
 __device__ __forceinline__ void book_energy(BondedEnergies& E, int kind, const TermForces& o) {
   if (kind == BK_BOND) E.bond += o.e;
   else if (kind == BK_ANGLE) E.angle += o.e;
-  else if (kind == BK_DIHEDRAL) E.dih += o.e;
+  else if (kind == BK_DIHEDRAL || kind == BK_CMAP) E.dih += o.e;  // CMAP energy is booked as dihedral energy
   else if (kind == BK_IMPROPER) E.imp += o.e;
   else E.lj += o.e, E.el += o.e2;
 }
@@ -143,11 +207,11 @@ __device__ __forceinline__ Vec3d bonded_force_on_atom(const DeviceState& S, cons
   const BoxView bx = box_of(S, r);
   Vec3d f = {0., 0., 0.};
   for (int p = T.atom_ptr[a]; p < T.atom_ptr[a + 1]; ++p) {
-    const unsigned ent = (unsigned)T.entries[p];
-    const int kind = ent >> 29, slot = (ent >> 27) & 3, t = ent & 0x7ffffff;
+    int kind, slot, t;
+    bonded_unpack((unsigned)T.entries[p], kind, slot, t);
     TermForces o;
     if (!bonded_term(S, T, q_scaled, pos, base, bx, kind, t, o)) continue;
-    f = f + (slot == 0 ? o.f[0] : (slot == 1 ? o.f[1] : (slot == 2 ? o.f[2] : o.f[3])));
+    f = f + (slot == 0 ? o.f[0] : (slot == 1 ? o.f[1] : (slot == 2 ? o.f[2] : (slot == 3 ? o.f[3] : o.f[4]))));
     if (slot == 0) book_energy(E, kind, o);
   }
   return f;
@@ -155,11 +219,13 @@ __device__ __forceinline__ Vec3d bonded_force_on_atom(const DeviceState& S, cons
 
 // Where the force of (kind, term, slot) sits in the per-term buffer: slots of a kind side by side
 struct TermLayout {
-  int first[5];  // first term index (over all kinds, in the order bonds, angles, dihedrals, impropers, 1-4) of each kind
-  int slot0[5];  // first buffer slot of each kind
+  int first[BK_KINDS];  // first term index (over all kinds, in the order bonds, angles, dihedrals, impropers, 1-4, CMAP) of each kind
+  int slot0[BK_KINDS];  // first buffer slot of each kind
   int nterms, nslots;
 };
-__host__ __device__ __forceinline__ int term_arity(int kind) { return kind == BK_ANGLE ? 3 : (kind == BK_DIHEDRAL || kind == BK_IMPROPER ? 4 : 2); }
+__host__ __device__ __forceinline__ int term_arity(int kind) {
+  return kind == BK_ANGLE ? 3 : (kind == BK_DIHEDRAL || kind == BK_IMPROPER ? 4 : (kind == BK_CMAP ? 5 : 2));
+}
 
 // block-level reduction of the bonded energies into the per-replica slots
 __device__ __forceinline__ void bonded_energy_reduce(const DeviceState& S, const BondedTables& T, int r, const BondedEnergies& E,
@@ -167,7 +233,7 @@ __device__ __forceinline__ void bonded_energy_reduce(const DeviceState& S, const
   double* Eo = energies + (size_t)r * TMD_NUM_ENERGIES;
   if (T.bonds.n) block_accumulate<BONDED_THREADS / 32>(E.bond, Eo + TMD_E_BONDS, red);
   if (T.angles.n) block_accumulate<BONDED_THREADS / 32>(E.angle, Eo + TMD_E_ANGLES, red);
-  if (T.torsions[0].n) block_accumulate<BONDED_THREADS / 32>(E.dih, Eo + TMD_E_DIHEDRALS, red);
+  if (T.torsions[0].n || T.cmap.n) block_accumulate<BONDED_THREADS / 32>(E.dih, Eo + TMD_E_DIHEDRALS, red);
   if (T.torsions[1].n) block_accumulate<BONDED_THREADS / 32>(E.imp, Eo + TMD_E_IMPROPERS, red);
   if (T.pairs14.n) {
     if (S.pp.terms & T_LJ) block_accumulate<BONDED_THREADS / 32>(E.lj, Eo + TMD_E_LJ, red);
@@ -183,9 +249,9 @@ k_bonded_terms(DeviceState S, BondedTables T, TermLayout lay, const float* __res
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
   BondedEnergies E;
   if (g < lay.nterms) {
-    int kind = BK_PAIR14;
+    int kind = BK_CMAP;
 #pragma unroll
-    for (int k = 3; k >= 0; --k)
+    for (int k = BK_KINDS - 2; k >= 0; --k)
       if (g < lay.first[k + 1]) kind = k;
     const int t = g - lay.first[kind];
     const size_t base = (size_t)r * S.natoms;
@@ -194,13 +260,13 @@ k_bonded_terms(DeviceState S, BondedTables T, TermLayout lay, const float* __res
     bool mine = S.own_all, books = S.own_all;
     if (!S.own_all) {
 #pragma unroll
-      for (int k = 0; k < 4; ++k) mine |= k < o.n && o.atom[k] >= S.own_lo && o.atom[k] < S.own_lo + S.own_n;
+      for (int k = 0; k < 5; ++k) mine |= k < o.n && o.atom[k] >= S.own_lo && o.atom[k] < S.own_lo + S.own_n;
       books = o.atom[0] >= S.own_lo && o.atom[0] < S.own_lo + S.own_n;
     }
     if (mine) {
       double* out = term_f + ((size_t)r * lay.nslots + lay.slot0[kind] + (size_t)t * o.n) * 3;
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
+      for (int k = 0; k < 5; ++k)
         if (k < o.n) {
           out[3 * k + 0] = acts ? o.f[k].x : 0.0;
           out[3 * k + 1] = acts ? o.f[k].y : 0.0;
@@ -227,8 +293,8 @@ k_bonded_sum(DeviceState S, BondedTables T, TermLayout lay, const double* __rest
   Vec3d f = {0., 0., 0.};
   const int p1 = T.atom_ptr[a + 1];
   for (int p = T.atom_ptr[a]; p < p1; ++p) {
-    const unsigned ent = (unsigned)T.entries[p];
-    const int kind = ent >> 29, slot = (ent >> 27) & 3, t = ent & 0x7ffffff;
+    int kind, slot, t;
+    bonded_unpack((unsigned)T.entries[p], kind, slot, t);
     const double* v = tf + ((size_t)lay.slot0[kind] + (size_t)t * term_arity(kind) + slot) * 3;
     f.x += v[0];
     f.y += v[1];

@@ -125,6 +125,16 @@ struct BondedSetT {
 };
 using BondedSet = BondedSetT<float>;
 
+// CMAP correction maps (tmd_set_cmap), one table for both precisions: n terms of 5 atoms, each on map map_of[t];
+// maps[m] = (first cell of map m in coef, resolution); 16 bicubic coefficients per cell (bonded.cuh, cmap_energy).
+struct CmapSet {
+  int n = 0;
+  int* idx = nullptr;      // (n,5)
+  int* map_of = nullptr;   // (n)
+  int2* maps = nullptr;    // (nmaps)
+  double* coef = nullptr;  // (cells,16)
+};
+
 // ---- "precision: double" (tmd_set_precision(ctx, 64)): full Verlet rows, fp64 state ------------
 // The list build is the fp32 one, run on an fp32 shadow of the positions (the list is a superset
 // of the pairs and decides nothing); the decision and every value are fp64.
@@ -165,6 +175,8 @@ struct tmd_ctx {
   float2* AB = nullptr;
   tmd::BondedSet bonds, angles, torsions[2], pairs14;
   std::vector<int32_t> bonds_idx_h, angles_idx_h, torsions_idx_h[2], pairs14_idx_h;  // host copies for the atom CSR
+  tmd::CmapSet cmap;                 // CMAP terms and maps (tmd_set_cmap), both precisions
+  std::vector<int32_t> cmap_idx_h;
   int* bonded_atom_ptr = nullptr;    // device CSR: atom -> bonded term entries (see bonded.cuh)
   int* bonded_entries = nullptr;
   int bonded_nentries = 0;

@@ -248,6 +248,7 @@ struct BondedTables64 {
   const int* atom_ptr;
   const int* entries;
   BondedSetT<double> bonds, angles, torsions[2], pairs14;
+  CmapSet cmap;
 };
 
 __device__ __forceinline__ Vec3d load3d(const double* p, size_t atom) {
@@ -306,6 +307,16 @@ __device__ __forceinline__ bool bonded_term_f64(const DeviceState& S, const Devi
     o.e = e;
     return true;
   }
+  if (kind == BK_CMAP) {
+    o.n = 5;
+#pragma unroll
+    for (int k = 0; k < 5; ++k) o.atom[k] = T.cmap.idx[5 * t + k];
+    const Vec3d p0 = load3d(pos, base + o.atom[0]), p1 = load3d(pos, base + o.atom[1]), p2 = load3d(pos, base + o.atom[2]);
+    const Vec3d p3 = load3d(pos, base + o.atom[3]), p4 = load3d(pos, base + o.atom[4]);
+    o.e = cmap_term(T.cmap, t, delta64(p0, p1, periodic, L), delta64(p1, p2, periodic, L), delta64(p2, p3, periodic, L),
+                    delta64(p3, p4, periodic, L), o.f);
+    return true;
+  }
   // BK_PAIR14 (forces.py:185-236): LJ/scnb with no cutoff or switch, Coulomb/scee, never RF
   const int i = T.pairs14.idx[2 * t], j = T.pairs14.idx[2 * t + 1];
   o.n = 2, o.atom[0] = i, o.atom[1] = j;
@@ -336,7 +347,7 @@ __device__ __forceinline__ void bonded_energy_reduce64(const DeviceState64& D, c
   double* Eo = energies + (size_t)r * TMD_NUM_ENERGIES;
   if (T.bonds.n) block_accumulate<BONDED_THREADS / 32>(E.bond, Eo + TMD_E_BONDS, red);
   if (T.angles.n) block_accumulate<BONDED_THREADS / 32>(E.angle, Eo + TMD_E_ANGLES, red);
-  if (T.torsions[0].n) block_accumulate<BONDED_THREADS / 32>(E.dih, Eo + TMD_E_DIHEDRALS, red);
+  if (T.torsions[0].n || T.cmap.n) block_accumulate<BONDED_THREADS / 32>(E.dih, Eo + TMD_E_DIHEDRALS, red);
   if (T.torsions[1].n) block_accumulate<BONDED_THREADS / 32>(E.imp, Eo + TMD_E_IMPROPERS, red);
   if (T.pairs14.n) {
     if (D.pp.terms & T_LJ) block_accumulate<BONDED_THREADS / 32>(E.lj, Eo + TMD_E_LJ, red);
@@ -351,16 +362,16 @@ k_bonded_terms_f64(DeviceState S, DeviceState64 D, BondedTables64 T, TermLayout 
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
   BondedEnergies E;
   if (g < lay.nterms) {
-    int kind = BK_PAIR14;
+    int kind = BK_CMAP;
 #pragma unroll
-    for (int k = 3; k >= 0; --k)
+    for (int k = BK_KINDS - 2; k >= 0; --k)
       if (g < lay.first[k + 1]) kind = k;
     const int t = g - lay.first[kind];
     TermForces o;
     const bool acts = bonded_term_f64(S, D, T, pos, r, kind, t, o);
     double* out = term_f + ((size_t)r * lay.nslots + lay.slot0[kind] + (size_t)t * o.n) * 3;
 #pragma unroll
-    for (int k = 0; k < 4; ++k)
+    for (int k = 0; k < 5; ++k)
       if (k < o.n) {
         out[3 * k + 0] = acts ? o.f[k].x : 0.0;
         out[3 * k + 1] = acts ? o.f[k].y : 0.0;
@@ -385,8 +396,8 @@ k_bonded_sum_f64(DeviceState S, BondedTables64 T, TermLayout lay, const double* 
   if (p1 == T.atom_ptr[a]) return;
   Vec3d f = {0., 0., 0.};
   for (int p = T.atom_ptr[a]; p < p1; ++p) {
-    const unsigned ent = (unsigned)T.entries[p];
-    const int kind = ent >> 29, slot = (ent >> 27) & 3, t = ent & 0x7ffffff;
+    int kind, slot, t;
+    bonded_unpack((unsigned)T.entries[p], kind, slot, t);
     const double* v = tf + ((size_t)lay.slot0[kind] + (size_t)t * term_arity(kind) + slot) * 3;
     f.x += v[0];
     f.y += v[1];

@@ -8,6 +8,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <string>
 #include <tuple>
 #include <utility>
@@ -331,7 +332,7 @@ const char* tmd_last_error(void) { return g_err.c_str(); }
 #if defined(TMD_SIMT_HOST)
 int tmd_version(void) { return -100; }  // host SIMT interpreter build (tests/simt): torchmd_b200/_lib.py refuses it
 #else
-int tmd_version(void) { return 104; }  // 101: the "precision: double" entry points (tmd_set_precision, *_f64); 102: constraints; 103: PME; 104: box rescale + molecule scaling
+int tmd_version(void) { return 105; }  // 101: the "precision: double" entry points (tmd_set_precision, *_f64); 102: constraints; 103: PME; 104: box rescale + molecule scaling; 105: CMAP
 #endif
 
 int tmd_create(tmd_ctx** out, int device, int natoms, int nreplicas) {
@@ -395,7 +396,7 @@ int tmd_destroy(tmd_ctx* ctx) {
                   ctx->bonds64.idx, ctx->bonds64.prm, ctx->angles64.idx, ctx->angles64.prm,
                   ctx->torsions64[0].idx, ctx->torsions64[0].term_ptr, ctx->torsions64[0].terms,
                   ctx->torsions64[1].idx, ctx->torsions64[1].term_ptr, ctx->torsions64[1].terms,
-                  ctx->pairs1464.idx, ctx->pairs1464.prm};
+                  ctx->pairs1464.idx, ctx->pairs1464.prm, ctx->cmap.idx, ctx->cmap.map_of, ctx->cmap.maps, ctx->cmap.coef};
   for (void* b : bufs)
     if (b) cudaFree(b);
   dd_release(ctx);
@@ -598,6 +599,114 @@ int tmd_set_torsions(tmd_ctx* ctx, int which, int n, const int32_t* idx, const i
   if (!ctx || which < 0 || which > 1) return fail(TMD_ERR_ARG, "tmd_set_torsions: bad arguments");
   TMD_PRECISION(ctx, 32, "tmd_set_torsions")
   return set_torsions(ctx, ctx->torsions[which], which, n, idx, term_ptr, terms, amber_form);
+}
+
+// ---- CMAP correction maps ------------------------------------------------------------------------
+// Derivatives, in grid units, of the periodic cubic spline through y[0], y[s], ..., y[(n-1)s]: d[k*s] = y'(k).
+// inv: first column of the inverse of the cyclic matrix (4 on the diagonal, 1 beside it) that gives the spline's
+// second derivatives M from 6 (y[k+1] - 2 y[k] + y[k-1]).
+static void periodic_spline_slopes(int n, const std::vector<double>& inv, const double* y, size_t s, double* d) {
+  std::vector<double> rhs(n), M(n, 0.0);
+  for (int k = 0; k < n; ++k) rhs[k] = 6.0 * (y[((k + 1) % n) * s] - 2.0 * y[k * s] + y[((k + n - 1) % n) * s]);
+  for (int i = 0; i < n; ++i)
+    for (int j = 0; j < n; ++j) M[i] += inv[(i - j + n) % n] * rhs[j];  // the inverse of a circulant matrix is circulant
+  for (int k = 0; k < n; ++k) d[k * s] = (y[((k + 1) % n) * s] - y[k * s]) - (2.0 * M[k] + M[(k + 1) % n]) / 6.0;
+}
+
+static std::vector<double> cyclic_spline_inverse(int n) {
+  std::vector<double> a((size_t)n * n, 0.0), x(n, 0.0);
+  for (int i = 0; i < n; ++i) {
+    a[(size_t)i * n + i] = 4.0;
+    a[(size_t)i * n + (i + 1) % n] += 1.0;
+    a[(size_t)i * n + (i + n - 1) % n] += 1.0;
+  }
+  x[0] = 1.0;
+  for (int c = 0; c < n; ++c) {  // Gaussian elimination; diagonally dominant, no pivoting needed
+    for (int r = c + 1; r < n; ++r) {
+      const double f = a[(size_t)r * n + c] / a[(size_t)c * n + c];
+      if (f == 0.0) continue;
+      for (int k = c; k < n; ++k) a[(size_t)r * n + k] -= f * a[(size_t)c * n + k];
+      x[r] -= f * x[c];
+    }
+  }
+  for (int r = n - 1; r >= 0; --r) {
+    double v = x[r];
+    for (int k = r + 1; k < n; ++k) v -= a[(size_t)r * n + k] * x[k];
+    x[r] = v / a[(size_t)r * n + r];
+  }
+  return x;
+}
+
+// Bicubic coefficients of every cell of one map (CHARMM's construction): dE/du and dE/dv from periodic splines along
+// each axis, d2E/dudv from a periodic spline along v of dE/du; per cell A = M F M^T, c[4p+q] the coefficient of u^p v^q.
+static void cmap_coefficients(int n, const double* E, double* out) {
+  const std::vector<double> inv = cyclic_spline_inverse(n);
+  const size_t nn = (size_t)n * n;
+  std::vector<double> du(nn), dv(nn), duv(nn);
+  for (int j = 0; j < n; ++j) periodic_spline_slopes(n, inv, E + j, n, du.data() + j);
+  for (int i = 0; i < n; ++i) periodic_spline_slopes(n, inv, E + (size_t)i * n, 1, dv.data() + (size_t)i * n);
+  for (int i = 0; i < n; ++i) periodic_spline_slopes(n, inv, du.data() + (size_t)i * n, 1, duv.data() + (size_t)i * n);
+  static const double Mx[4][4] = {{1, 0, 0, 0}, {0, 0, 1, 0}, {-3, 3, -2, -1}, {2, -2, 1, 1}};
+  for (int i = 0; i < n; ++i)
+    for (int j = 0; j < n; ++j) {
+      const int i1 = (i + 1) % n, j1 = (j + 1) % n;
+      auto at = [&](const std::vector<double>& g, int a, int b) { return g[(size_t)a * n + b]; };
+      auto e = [&](int a, int b) { return E[(size_t)a * n + b]; };
+      const double F[4][4] = {{e(i, j), e(i, j1), at(dv, i, j), at(dv, i, j1)},
+                              {e(i1, j), e(i1, j1), at(dv, i1, j), at(dv, i1, j1)},
+                              {at(du, i, j), at(du, i, j1), at(duv, i, j), at(duv, i, j1)},
+                              {at(du, i1, j), at(du, i1, j1), at(duv, i1, j), at(duv, i1, j1)}};
+      double MF[4][4];
+      for (int p = 0; p < 4; ++p)
+        for (int q = 0; q < 4; ++q) {
+          MF[p][q] = 0.0;
+          for (int k = 0; k < 4; ++k) MF[p][q] += Mx[p][k] * F[k][q];
+        }
+      double* c = out + ((size_t)i * n + j) * 16;
+      for (int p = 0; p < 4; ++p)
+        for (int q = 0; q < 4; ++q) {
+          double v = 0.0;
+          for (int k = 0; k < 4; ++k) v += MF[p][k] * Mx[q][k];
+          c[4 * p + q] = v;
+        }
+    }
+}
+
+constexpr int CMAP_MAX_RES = 360;  // (the host spline set-up is O(res^3) per map)
+
+int tmd_set_cmap(tmd_ctx* ctx, int nmaps, const int32_t* res, const double* grids, int n, const int32_t* idx,
+                 const int32_t* map_of) {
+  if (!ctx || nmaps < 0 || n < 0 || (nmaps > 0 && (!res || !grids)) || (n > 0 && (!idx || !map_of)))
+    return fail(TMD_ERR_ARG, "tmd_set_cmap: bad arguments");
+  if (n > 0 && nmaps == 0) return fail(TMD_ERR_ARG, "tmd_set_cmap: terms without maps");
+  DeviceGuard guard(ctx->device);
+  std::vector<int2> maps(nmaps);
+  long long cells = 0;
+  for (int m = 0; m < nmaps; ++m) {
+    if (res[m] < 4 || res[m] > CMAP_MAX_RES) return fail(TMD_ERR_ARG, "tmd_set_cmap: map resolution outside 4..360");
+    maps[m] = make_int2((int)cells, res[m]);
+    cells += (long long)res[m] * res[m];
+    if (cells * 16 >= (1ll << 31)) return fail(TMD_ERR_ARG, "tmd_set_cmap: maps too large");
+  }
+  for (long long k = 0; k < cells; ++k)
+    if (!std::isfinite(grids[k])) return fail(TMD_ERR_ARG, "tmd_set_cmap: grid value not finite");
+  for (long long e = 0; e < (long long)n * 5; ++e)
+    if (idx[e] < 0 || idx[e] >= ctx->natoms) return fail(TMD_ERR_ARG, "tmd_set_cmap: atom index out of range");
+  for (int t = 0; t < n; ++t)
+    if (map_of[t] < 0 || map_of[t] >= nmaps) return fail(TMD_ERR_ARG, "tmd_set_cmap: map index out of range");
+  std::vector<double> coef((size_t)cells * 16);
+  for (int m = 0; m < nmaps; ++m) cmap_coefficients(maps[m].y, grids + maps[m].x, coef.data() + (size_t)maps[m].x * 16);
+  CmapSet& C = ctx->cmap;
+  int rc;
+  if ((rc = upload(&C.idx, idx, (size_t)n * 5))) return rc;
+  if ((rc = upload(&C.map_of, map_of, (size_t)n))) return rc;
+  if ((rc = upload(&C.maps, maps.data(), maps.size()))) return rc;
+  if ((rc = upload(&C.coef, coef.data(), coef.size()))) return rc;
+  C.n = n;
+  ctx->cmap_idx_h.assign(idx, idx + (size_t)n * 5);
+  ctx->touched = true;
+  priv(ctx).dirty = true;
+  return TMD_OK;
 }
 
 // ---- "precision: double" --------------------------------------------------------------------
@@ -1184,12 +1293,13 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   {
     const uint32_t bm = ctx->bonded_mask;
     struct Src { int kind, k; const std::vector<int32_t>* idx; bool on; };
-    const Src src[5] = {
+    const Src src[6] = {
         {BK_BOND, 2, &ctx->bonds_idx_h, (bm & TMD_TERM(TMD_E_BONDS)) != 0},
         {BK_ANGLE, 3, &ctx->angles_idx_h, (bm & TMD_TERM(TMD_E_ANGLES)) != 0},
         {BK_DIHEDRAL, 4, &ctx->torsions_idx_h[0], (bm & TMD_TERM(TMD_E_DIHEDRALS)) != 0},
         {BK_PAIR14, 2, &ctx->pairs14_idx_h, (bm & TMD_TERM(TMD_E_14)) != 0},
-        {BK_IMPROPER, 4, &ctx->torsions_idx_h[1], (bm & TMD_TERM(TMD_E_IMPROPERS)) != 0}};
+        {BK_IMPROPER, 4, &ctx->torsions_idx_h[1], (bm & TMD_TERM(TMD_E_IMPROPERS)) != 0},
+        {BK_CMAP, 5, &ctx->cmap_idx_h, (bm & TMD_TERM(TMD_E_DIHEDRALS)) != 0}};  // CMAP acts with the dihedrals
     std::vector<int> ptr(N + 1, 0);
     for (const Src& sc : src)
       if (sc.on)
@@ -1199,10 +1309,10 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
     for (const Src& sc : src) {
       if (!sc.on) continue;
       const size_t nt = sc.idx->size() / sc.k;
-      if (nt >= (1u << 27)) return fail(TMD_ERR_UNSUPPORTED, "more than 2^27 bonded terms of one kind");
+      if (nt >= (1u << 26)) return fail(TMD_ERR_UNSUPPORTED, "more than 2^26 bonded terms of one kind");
       for (size_t t = 0; t < nt; ++t)
         for (int sl = 0; sl < sc.k; ++sl)
-          ent[fill[(*sc.idx)[t * sc.k + sl]]++] = (int)(((unsigned)sc.kind << 29) | ((unsigned)sl << 27) | (unsigned)t);
+          ent[fill[(*sc.idx)[t * sc.k + sl]]++] = (int)bonded_entry(sc.kind, sl, (unsigned)t);
     }
     ctx->bonded_nentries = ptr[N];
     if ((rc = upload(&ctx->bonded_atom_ptr, ptr.data(), ptr.size()))) return rc;
@@ -1383,9 +1493,10 @@ static Tables bonded_tables(const tmd_ctx* ctx, const Set& bonds, const Set& ang
   T.torsions[0] = torsions[0];
   T.torsions[1] = torsions[1];
   T.pairs14 = pairs14;
+  T.cmap = ctx->cmap;
   if (!(bm & TMD_TERM(TMD_E_BONDS))) T.bonds.n = 0;
   if (!(bm & TMD_TERM(TMD_E_ANGLES))) T.angles.n = 0;
-  if (!(bm & TMD_TERM(TMD_E_DIHEDRALS))) T.torsions[0].n = 0;
+  if (!(bm & TMD_TERM(TMD_E_DIHEDRALS))) T.torsions[0].n = 0, T.cmap.n = 0;
   if (!(bm & TMD_TERM(TMD_E_IMPROPERS))) T.torsions[1].n = 0;
   if (!(bm & TMD_TERM(TMD_E_14))) T.pairs14.n = 0;
   return T;
@@ -1394,9 +1505,9 @@ static Tables bonded_tables(const tmd_ctx* ctx, const Set& bonds, const Set& ang
 template <typename Tables>
 static TermLayout term_layout(const Tables& T) {
   TermLayout lay;
-  const int cnt[5] = {T.bonds.n, T.angles.n, T.torsions[0].n, T.torsions[1].n, T.pairs14.n};
+  const int cnt[BK_KINDS] = {T.bonds.n, T.angles.n, T.torsions[0].n, T.torsions[1].n, T.pairs14.n, T.cmap.n};
   int nt = 0, ns = 0;
-  for (int k = 0; k < 5; ++k) {
+  for (int k = 0; k < BK_KINDS; ++k) {
     lay.first[k] = nt;
     lay.slot0[k] = ns;
     nt += cnt[k];

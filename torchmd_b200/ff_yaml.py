@@ -9,6 +9,7 @@ with positions permuted around the improper centre (impropers, position 2); the 
 fewest wildcards wins, ties resolved in the reference's enumeration order.
 """
 import math
+import warnings
 from itertools import permutations, product
 
 import numpy as np
@@ -102,7 +103,12 @@ def yaml_parameters(mol, forcefield, terms=None, precision=torch.float32, device
     (path, dict or YamlForceField): the reference's ``Parameters(YamlForcefield(mol, yaml), mol,
     terms)`` -- same unique-term ordering, same first-appearance parameter rows.  Like the
     reference (``torch.tensor(list of Python floats)`` is fp32, then ``.type(precision)``) every
-    parameter value passes through fp32, also for ``precision=torch.float64``."""
+    parameter value passes through fp32, also for ``precision=torch.float64``.
+
+    ``"cmap"`` in ``terms`` (not among the defaults) builds CMAP terms from the molecule's ``crossterms`` (C,8) with a
+    force field that has ``get_cmap`` (charmm.CharmmPrmForceField); without it they are left out with a warning.  A
+    cross-term must be two dihedrals that share three atoms, (a,b,c,d) and (b,c,d,e), as every backbone phi/psi pair
+    is; it becomes the 5-atom term (a,b,c,d,e).  The grids keep the file's values (fp64)."""
     # a force-field object with the reference's interface (YamlForceField, charmm.CharmmPrmForceField), or a YAML path / dict
     ff = forcefield if hasattr(forcefield, "get_LJ") else YamlForceField(forcefield)
     if terms is None:
@@ -199,6 +205,25 @@ def yaml_parameters(mol, forcefield, terms=None, precision=torch.float32, device
                     rows.append([ep * 4 * s6 * s6, ep * 4 * s6, scnb, scee])
                 pmap.append([i, row_of[key]])
             pairs14 = (d14[:, [0, 3]], np.array(pmap, dtype=np.int64), _f32(rows))
+    cross, cmaps = arr("crossterms", 8), None
+    if len(cross) and "cmap" not in terms:
+        warnings.warn(f"the molecule has {len(cross)} CMAP cross-terms; they are left out unless terms includes 'cmap'",
+                      stacklevel=2)
+    elif len(cross):
+        if not hasattr(ff, "get_cmap"):
+            raise RuntimeError("'cmap' was asked for, but the force field holds no CMAP maps")
+        bad = np.any(cross[:, 1:4] != cross[:, 4:7], axis=1)
+        if bad.any():
+            raise ValueError(f"cross-term {cross[np.argmax(bad)].tolist()} is not two dihedrals (a,b,c,d), (b,c,d,e): "
+                             "only that 5-atom form is supported")
+        grids, map_of, map_ix = [], [], {}
+        for row in cross:
+            key = tuple(T[row])
+            if key not in map_ix:
+                map_ix[key] = len(grids)
+                grids.append(np.asarray(ff.get_cmap(key), dtype=np.float64))
+            map_of.append(map_ix[key])
+        cmaps = (cross[:, [0, 1, 2, 3, 7]], np.array(map_of, np.int64), [len(g) for g in grids], grids)
     return TopologyParameters(
         atom_types=types,
         type_sigma=sigma,
@@ -210,6 +235,7 @@ def yaml_parameters(mol, forcefield, terms=None, precision=torch.float32, device
         dihedrals=dihedrals,
         impropers=impropers,
         pairs14=pairs14,
+        cmaps=cmaps,
         precision=precision,
         device=device,
     )

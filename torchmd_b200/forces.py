@@ -56,7 +56,9 @@ class Forces:
     Parameters
     ----------
     parameters : object with the reference ``Parameters`` attribute layout
-    terms : list of str, case-insensitive, from ``Forces.terms``
+    terms : list of str, case-insensitive, from ``Forces.terms``.  ``"dihedrals"`` also turns on the CMAP
+        correction maps the parameters carry (``cmap_params``, built by the parameter builders when asked for
+        ``"cmap"``); their energy is part of the ``dihedrals`` energy.
     external : optional plugin exposing ``calculate(pos, box) -> (E (R,), F (R,N,3))``
     cutoff, rfa, solventDielectric, switch_dist, exclusions : as in the reference
     skin : Verlet-list buffer in Angstrom (not in the reference; results do not depend on it)
@@ -277,6 +279,11 @@ class Forces:
         if "1-4" in self.energies and par.nonbonded_14_params is not None and len(par.nonbonded_14_params["idx"]):
             idx, _, prm = instance_rows(par.nonbonded_14_params)
             check(setter("tmd_set_pairs14")(ctx, len(idx), _lib.ptr(idx), _lib.ptr(prm)))
+        cmap = getattr(par, "cmap_params", None)  # (a reference Parameters object has none)
+        if "dihedrals" in self.energies and cmap is not None and len(cmap["idx"]):
+            res, grids = _np(cmap["res"], np.int32), _np(cmap["grids"], np.float64)
+            idx, map_of = _np(cmap["idx"], np.int32), _np(cmap["map_of"], np.int32)
+            check(L.tmd_set_cmap(ctx, len(res), _lib.ptr(res), _lib.ptr(grids), len(idx), _lib.ptr(idx), _lib.ptr(map_of)))
 
     def _ensure_box(self, box):
         """Hand the box diagonal to the context when the tensor changed (one D2H copy).  The tensor the

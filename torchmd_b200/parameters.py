@@ -11,6 +11,11 @@ same attribute names that is filled straight from arrays.  A reference
 Layout (per term ``bond/angle/dihedral/improper/nonbonded_14``):
 ``{"idx": (M,k) int64, "map": (M',2) int64 [row -> param row], "params": (K,p)}``
 with p = 2 (k, r0 | k, theta0 rad), 3 (k, phi0 rad, periodicity), 4 (A, B, scnb, scee).
+
+CMAP correction maps (not in the reference) are ``cmap_params = {"idx": (n,5) int64, "map_of": (n,) int64,
+"res": (nmaps,) int64, "grids": (sum res^2,) float64}``: term t acts on atoms idx[t] with phi = dihedral(idx[t,0:4]),
+psi = dihedral(idx[t,1:5]) and map map_of[t]; map m holds E(phi_i, psi_j) at phi_i = -180 deg + i 360 deg / res[m]
+(psi alike), phi-major, in kcal/mol.  The grids stay fp64 in both precisions.
 """
 import numpy as np
 import torch
@@ -40,6 +45,22 @@ def _term(idx, pmap, params, dtype):
     return {"idx": idx, "map": pmap, "params": params}
 
 
+def _cmap(idx, map_of, res, grids, natoms):
+    idx = torch.as_tensor(np.asarray(idx, dtype=np.int64).reshape(-1, 5))
+    map_of = torch.as_tensor(np.asarray(map_of, dtype=np.int64).reshape(-1))
+    res = torch.as_tensor(np.asarray(res, dtype=np.int64).reshape(-1))
+    if isinstance(grids, (list, tuple)):  # one (res, res) grid per map
+        grids = np.concatenate([np.ravel(np.asarray(g, dtype=np.float64)) for g in grids])
+    grids = torch.as_tensor(np.ravel(np.asarray(grids, dtype=np.float64)))
+    if len(map_of) != len(idx) or int(map_of.min()) < 0 or int(map_of.max()) >= len(res):
+        raise ValueError("cmaps: map_of must give one map index in 0..nmaps-1 per term")
+    if int(idx.min()) < 0 or int(idx.max()) >= natoms:
+        raise ValueError("cmaps: atom index out of range")
+    if int((res * res).sum()) != len(grids):
+        raise ValueError(f"cmaps: the grids hold {len(grids)} values, the resolutions need {int((res * res).sum())}")
+    return {"idx": idx, "map_of": map_of, "res": res, "grids": grids}
+
+
 class TopologyParameters:
     """Array-built stand-in for the reference ``Parameters`` object."""
 
@@ -55,6 +76,7 @@ class TopologyParameters:
         dihedrals=None,
         impropers=None,
         pairs14=None,
+        cmaps=None,
         precision=torch.float32,
         device="cpu",
     ):
@@ -64,6 +86,7 @@ class TopologyParameters:
         charges, masses : (N,)
         bonds/angles/dihedrals/impropers/pairs14 : optional ``(idx, map, params)``
             triples in the layout described in the module docstring.
+        cmaps : optional ``(idx (n,5), map_of (n,), res (nmaps,), grids)`` CMAP terms and maps (module docstring)
         """
         self.natoms = int(len(atom_types))
         self.mapped_atom_types = torch.as_tensor(
@@ -87,6 +110,7 @@ class TopologyParameters:
         self.dihedral_params = _term(*dihedrals, torch.float64) if dihedrals else None
         self.improper_params = _term(*impropers, torch.float64) if impropers else None
         self.nonbonded_14_params = _term(*pairs14, torch.float64) if pairs14 else None
+        self.cmap_params = _cmap(*cmaps, self.natoms) if cmaps is not None and len(cmaps[0]) else None
         self.A = None
         self.B = None
         self.device = "cpu"
@@ -112,6 +136,8 @@ class TopologyParameters:
             if t is not None:
                 for k in t:
                     t[k] = t[k].to(device)
+        if self.cmap_params is not None:
+            self.cmap_params = {k: v.to(device) for k, v in self.cmap_params.items()}
         if self.A is not None:
             self.A, self.B = self.A.to(device), self.B.to(device)
         self.device = device
