@@ -377,7 +377,8 @@ int tmd_export_pairs(tmd_ctx* ctx, const float* pos_dev, int replica, int32_t* p
  * default), 1 k_pair_fx (fixed-point separations), 2 k_pair_fx2 (fixed point + fp32x2
  * arithmetic), 3 k_pair2_open (no box, fp32x2 arithmetic), 4 k_cpair (cluster lists),
  * 5 k_pair_f64 (fp64 context); with particle-mesh Ewald, the real-space Ewald instantiations
- * 6 k_pair<MODE 2>, 7 k_pair_fx<MODE 2>, 8 k_ewpair64 (fp64).  For tests and bench labels. */
+ * 6 k_pair<MODE 2>, 7 k_pair_fx<MODE 2>, 8 k_ewpair64 (fp64), 9 k_pair_fx2_ew, 10 k_cpair_ew
+ * (cluster lists).  For tests and bench labels. */
 int tmd_pair_kernel(tmd_ctx* ctx);
 
 typedef struct {

@@ -58,8 +58,9 @@ constexpr int CL_WARPS = CL_WARPS_N;
 constexpr int CL_UNROLL_N = CL_UNROLL;
 constexpr int CLB_WARPS = 4;   // list build: warps per CTA
 constexpr int CLB_MAXSEG = 160;
-constexpr int CL_SIMT_MAX_ENTRIES = 4096;  // interpreter build (tests/simt): entries per cluster its static buffer holds
-constexpr int CL_SIMT_MAX_TYPES = 64;       // ... and atom types its static table holds
+// dynamic shared memory of k_cpair / k_cpair_ew (entry buffers + LJ table): a context whose lists would need more takes
+// the full rows (finalize); the interpreter build (tests/simt) holds exactly this much in a static buffer
+constexpr size_t CL_SMEM_MAX = (size_t)180 * 1024;
 
 __device__ __forceinline__ size_t cl_slot_base(const ClusterState& C, int r) { return (size_t)r * (C.slots + 1); }
 __device__ __forceinline__ size_t cl_cluster_base(const ClusterState& C, int r) { return (size_t)r * C.nclusters_cap; }
@@ -701,7 +702,7 @@ __device__ __noinline__ float2 cl_exact_pass_ew(ClExactArgs a, int2 mt, SwitchCo
 template <bool ENERGY, bool PERIODIC, bool EW>
 __device__ __forceinline__ void cpair_body(const DeviceState& S, const SwitchConsts& sc, double* __restrict__ energies) {
 #if defined(TMD_SIMT_HOST)
-  __shared__ __attribute__((aligned(128))) unsigned char cl_dyn[CL_WARPS * 2 * CL_SIMT_MAX_ENTRIES * 5 + CL_WARPS * CL_SIMT_MAX_TYPES * CL_H * sizeof(ClTab)];  // (interpreter build: no dynamic window)
+  __shared__ __attribute__((aligned(128))) unsigned char cl_dyn[CL_SMEM_MAX];  // (interpreter build: no dynamic window)
 #else
   extern __shared__ __align__(128) unsigned char cl_dyn[];
 #endif

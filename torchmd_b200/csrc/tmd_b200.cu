@@ -1052,6 +1052,29 @@ static bool box_grid(tmd_ctx* ctx, Grid& g, const float* L3, double rl, double m
 // list radius margin (A) over cutoff + skin: see finalize
 static double list_margin(const tmd_ctx* ctx) { return 0.004 + (ctx->precision == 64 ? 36.0 / 4096.0 : 0.0); }
 
+// Cluster-list capacities per cluster (ecap plain entries, mcap masked entries) and the dynamic shared memory k_cpair
+// stages them in: per warp two entry buffers of (mcap + ecap) words plus mcap mask bytes, then per warp the LJ table
+// (cluster.cuh, cpair_body).  keep_ecap / keep_mcap: capacities already reached (0: none), which are never lowered.
+struct ClSizing {
+  int ecap, mcap;
+  size_t smem;
+};
+static ClSizing cluster_sizing(const tmd_ctx* ctx, double rl, int nsub, double max_density, int keep_ecap, int keep_mcap) {
+  const int N = ctx->natoms;
+  // entries per cluster: half of the atoms within rl of a box of about (2.5, w, w) A, with head room
+  const double w = rl / nsub, a = 2.5, rho = std::max(max_density, 0.11);
+  const double vol = a * w * w + 2.0 * (a * w + w * w + a * w) * rl + M_PI * (a + 2 * w) * rl * rl + 4.0 / 3.0 * M_PI * rl * rl * rl;
+  long long ecap = (long long)(0.5 * rho * vol * 1.6) + 128;
+  if (const char* e = getenv("TMD_B200_CLUSTER_ECAP")) ecap = std::max(32, atoi(e));  // (tests: start too small, grow)
+  ecap = std::max<long long>(ecap, keep_ecap);
+  ecap = std::min<long long>((ecap + 31) / 32 * 32, ((long long)N + 31) / 32 * 32);
+  ClSizing s;
+  s.ecap = (int)std::max<long long>(ecap, 32);
+  s.mcap = std::max(64, keep_mcap);
+  s.smem = (size_t)CL_WARPS * 2 * ((size_t)(s.mcap + s.ecap) * sizeof(unsigned) + s.mcap) + (size_t)CL_WARPS * ctx->d.ntypes * CL_H * sizeof(ClTab);
+  return s;
+}
+
 static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   if (!ctx->have_atoms) return fail(TMD_ERR_STATE, "tmd_set_atoms has not been called");
   if (!ctx->have_box) return fail(TMD_ERR_STATE, "tmd_set_box has not been called");
@@ -1121,7 +1144,28 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
     cl_max_extent = 0.5 * (double)lmin - rl - ctx->skin - 0.05;
     use_cluster = cl_max_extent >= cl_extent;
   }
-  d.nsub = use_cluster ? std::max(1, (int)floor(rl / 4.0 + 0.5)) : 2;  // cluster path: cells of about 4 A
+  double max_density = 0.0;  // atoms per A^3 of the densest replica box
+  if (ctx->periodic)
+    for (int r = 0; r < R; ++r)
+      max_density = std::max(max_density, N / ((double)ctx->box_host[r * 3] * ctx->box_host[r * 3 + 1] * ctx->box_host[r * 3 + 2]));
+  const int cl_nsub = std::max(1, (int)floor(rl / 4.0 + 0.5));  // cluster path: cells of about 4 A
+  ClSizing cl_size{};
+  if (use_cluster) {
+    // the lists must fit k_cpair's shared-memory staging (long cutoffs, many atom types): otherwise the full rows.  When
+    // only the capacities grown after an overflow do not fit, the context gives up the cluster lists as after F_CLFAIL
+    // and tries them again later with fresh capacities.
+    const ClSizing fresh = cluster_sizing(ctx, rl, cl_nsub, max_density, 0, 0);
+    cl_size = cluster_sizing(ctx, rl, cl_nsub, max_density, cl.ecap, cl.mcap);
+    if (fresh.smem > CL_SMEM_MAX) {
+      use_cluster = false;
+    } else if (cl_size.smem > CL_SMEM_MAX) {
+      use_cluster = false;
+      ctx->cluster_failed = true;
+      ctx->cluster_retry_after = std::min<int64_t>(std::max<int64_t>(2 * ctx->cluster_retry_after, 1000), 1 << 20);
+      ctx->cluster_retry_at = ctx->force_calls + ctx->cluster_retry_after;
+    }
+  }
+  d.nsub = use_cluster ? cl_nsub : 2;
 
   // guard-free minimum image is valid iff no listed pair can be further than 0.45 L apart
   ctx->safe_image = false;
@@ -1142,12 +1186,10 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   // cell grid per replica
   std::vector<Grid> grids(R);
   long long max_cells = 1;
-  double max_density = 0.0;
   for (int r = 0; r < R; ++r) {
     Grid& g = grids[r];
     box_grid(ctx, g, &ctx->box_host[r * 3], rl, margin, nullptr);
     max_cells = std::max<long long>(max_cells, g.ncells);
-    if (ctx->periodic) max_density = std::max(max_density, N / ((double)g.L[0] * g.L[1] * g.L[2]));
   }
   if (!ctx->periodic && has_cut) max_cells = use_cluster ? 40 * 40 * 40 : 64 * 64 * 64;  // (cluster path: a bucket per cell)
   d.max_cells = (int)max_cells;
@@ -1190,7 +1232,6 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   // cluster path: slot arrays and lists
   {
     CtxPriv& pv = priv(ctx);
-    const int keep_ecap = cl.ecap, keep_mcap = cl.mcap;
     for (void* b : pv.cl_bufs) cudaFree(b);
     pv.cl_bufs.clear();
     memset(&cl, 0, sizeof(cl));
@@ -1204,15 +1245,8 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
       cl.slots = (int)slots;
       cl.nclusters_cap = (int)(slots / CL);
       cl.max_extent = (float)cl_max_extent;
-      // entries per cluster: half of the atoms within rl of a box of about (2.5, w, w) A, with head room
-      const double w = rl / d.nsub, a = 2.5, rho = std::max(max_density, 0.11);
-      const double vol = a * w * w + 2.0 * (a * w + w * w + a * w) * rl + M_PI * (a + 2 * w) * rl * rl + 4.0 / 3.0 * M_PI * rl * rl * rl;
-      long long ecap = (long long)(0.5 * rho * vol * 1.6) + 128;
-      if (const char* e = getenv("TMD_B200_CLUSTER_ECAP")) ecap = std::max(32, atoi(e));  // (tests: start too small, grow)
-      ecap = std::max<long long>(ecap, keep_ecap);
-      ecap = std::min<long long>((ecap + 31) / 32 * 32, ((long long)N + 31) / 32 * 32);
-      cl.ecap = (int)std::max<long long>(ecap, 32);
-      cl.mcap = std::max(64, keep_mcap);
+      cl.ecap = cl_size.ecap;
+      cl.mcap = cl_size.mcap;
       auto grab = [&](auto** ptr, size_t n) {
         void* b = nullptr;
         if (cudaMalloc(&b, n * sizeof(**ptr)) != cudaSuccess) return false;
@@ -1244,9 +1278,8 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
         TMD_CUDA(cudaMemcpy(cl.inv, ident.data(), ident.size() * sizeof(int), cudaMemcpyHostToDevice));
       }
       // launch shape of k_cpair: persistent CTAs, as many as fit
-      pv.cl_smem = (size_t)CL_WARPS * 2 * ((size_t)(cl.mcap + cl.ecap) * sizeof(unsigned) + cl.mcap) + (size_t)CL_WARPS * d.ntypes * CL_H * sizeof(ClTab);
+      pv.cl_smem = cl_size.smem;  // (at most CL_SMEM_MAX: decided above)
 #if !defined(TMD_SIMT_HOST)
-      if (pv.cl_smem > (size_t)180 * 1024) return fail(TMD_ERR_UNSUPPORTED, "cluster lists too long for the shared-memory staging");
       int per_sm = 0;
       const void* kernels[6] = {(const void*)k_cpair<false, false>, (const void*)k_cpair<false, true>,
                                 (const void*)k_cpair<true, false>, (const void*)k_cpair<true, true>,
@@ -1255,7 +1288,6 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
       TMD_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cpair<false, true>, CL_WARPS * 32, pv.cl_smem));
       pv.cl_blocks = std::max(1, std::min(ctx->nsm * std::max(per_sm, 1), (cl.nclusters_cap + CL_WARPS - 1) / CL_WARPS));
 #else
-      if (cl.mcap + cl.ecap > CL_SIMT_MAX_ENTRIES || d.ntypes > CL_SIMT_MAX_TYPES) return fail(TMD_ERR_UNSUPPORTED, "interpreter build: cluster list too long");
       pv.cl_blocks = std::max(1, std::min(16, (cl.nclusters_cap + CL_WARPS - 1) / CL_WARPS));
 #endif
     }
