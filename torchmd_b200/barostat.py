@@ -182,8 +182,9 @@ class MonteCarloBarostat:
         f._box_ref = box
 
     def attempt(self, ctx, energies):
-        """One move of every replica from the state whose (R, NUM_ENERGIES) device energies are ``energies``.
-        Returns the per-replica potential energies (host floats) of the state it leaves."""
+        """One move of every replica from the state whose (R, NUM_ENERGIES) device energies are ``energies``; an
+        accepted replica's row is overwritten with the energies of its new state.  Returns the per-replica potential
+        energies (host floats) of the state it leaves."""
         integ = self._integ
         s, f = integ.systems, integ.forces
         L = _lib.lib()
@@ -239,6 +240,7 @@ class MonteCarloBarostat:
         for r in range(nrep):  # (per replica slices: no mask, no host round trip)
             if ok[r]:
                 s.forces[r].copy_(trial_f[r])
+                energies[r].copy_(ene[r])  # the per-term energies the caller holds describe the state it leaves
             else:
                 s.pos[r].copy_(saved[r])
                 if saved_vel is not None:

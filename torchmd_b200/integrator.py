@@ -261,7 +261,9 @@ class Integrator:
         if self.batch is None:
             Ekin = ke.cpu().numpy().astype(np.float64 if f64 else np.float32)  # the state's dtype, like integrator.py:122-125
         else:
-            Ekin = kinetic_energy(self.masses, s.vel, self.batch).flatten().cpu().numpy()
+            # summed in fp64 like the kernels' ke, then given the state's dtype
+            Ekin = kinetic_energy(self.masses.double(), s.vel.double(), self.batch).flatten().cpu().numpy()
+            Ekin = Ekin.astype(np.float64 if f64 else np.float32)
         if self.constraints is None:
             T = kinetic_to_temp(Ekin, self.natoms)
         else:
