@@ -46,7 +46,7 @@ enum {
 /* Energy slots, in the order of torchmd Forces.terms (forces.py:23-25). */
 enum {
   TMD_E_BONDS = 0,
-  TMD_E_ANGLES = 1,
+  TMD_E_ANGLES = 1, /* angles plus the Urey-Bradley 1-3 terms (tmd_set_urey_bradley) */
   TMD_E_DIHEDRALS = 2, /* proper dihedrals plus the CMAP correction maps (tmd_set_cmap) */
   TMD_E_IMPROPERS = 3,
   TMD_E_14 = 4, /* stays 0: 1-4 energies are booked under lj/electrostatics, forces.py:185-236 */
@@ -112,6 +112,14 @@ int tmd_set_pairs14(tmd_ctx* ctx, int n, const int32_t* idx_host, const float* p
  * fp64).  n = 0 clears the terms. */
 int tmd_set_cmap(tmd_ctx* ctx, int nmaps, const int32_t* res_host, const double* grids_host,
                  int n, const int32_t* idx_host, const int32_t* map_of_host);
+
+/* Urey-Bradley 1-3 terms (library version >= 106; no reference counterpart).  n terms, idx (n,2) =
+ * the two end atoms of an angle, prm (n,2) = k_ub [kcal/mol/A^2], s0 [A]; E = k_ub (r13 - s0)^2,
+ * evaluated in fp64 with the minimum image and never cutoff-filtered.  Energies are booked in
+ * TMD_E_ANGLES; the terms act when the angle bit of the term mask is set.  TMD_ERR_ARG for an atom
+ * out of range, i == j, a negative or non-finite k_ub or a non-finite s0.  n = 0 clears the terms.
+ * tmd_set_urey_bradley_f64 is the same for contexts of tmd_set_precision(ctx, 64). */
+int tmd_set_urey_bradley(tmd_ctx* ctx, int n, const int32_t* idx_host, const float* prm_host);
 
 /* Box diagonal per replica, host (nreplicas,3).  All zeros = no periodic
  * wrapping (forces.py:361).  Sizes the cell grid; call again if the box changes. [sync] */
@@ -257,6 +265,7 @@ int tmd_set_angles_f64(tmd_ctx* ctx, int n, const int32_t* idx_host, const doubl
 int tmd_set_torsions_f64(tmd_ctx* ctx, int which, int n, const int32_t* idx_host,
                          const int32_t* term_ptr_host, const double* terms_host, int amber_form);
 int tmd_set_pairs14_f64(tmd_ctx* ctx, int n, const int32_t* idx_host, const double* prm_host);
+int tmd_set_urey_bradley_f64(tmd_ctx* ctx, int n, const int32_t* idx_host, const double* prm_host);
 int tmd_set_box_f64(tmd_ctx* ctx, const double* box_diag_host);
 int tmd_forces_f64(tmd_ctx* ctx, const double* pos_dev, double* forces_dev, double* energies_dev,
                    tmd_stream stream);

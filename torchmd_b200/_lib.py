@@ -118,6 +118,9 @@ _SIGNATURES = {
     "tmd_rewind_noise": (C.c_int, [_P, C.c_int, _P]),
     # CMAP correction maps (library version >= 105)
     "tmd_set_cmap": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, _P, _P]),
+    # Urey-Bradley terms (library version >= 106)
+    "tmd_set_urey_bradley": (C.c_int, [_P, C.c_int, _P, _P]),
+    "tmd_set_urey_bradley_f64": (C.c_int, [_P, C.c_int, _P, _P]),
 }
 ERR_UNSUPPORTED = -5
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
@@ -136,8 +139,8 @@ def lib():
                 "torchmd_b200 has no CPU or PyTorch fallback."
             )
         handle = C.CDLL(LIB_PATH)
-        if not hasattr(handle, "tmd_set_cmap"):
-            raise ImportError(f"{LIB_PATH} predates the CMAP entry point: rebuild it (__graft_entry__.build())")
+        if not hasattr(handle, "tmd_set_urey_bradley"):
+            raise ImportError(f"{LIB_PATH} predates the Urey-Bradley entry points: rebuild it (__graft_entry__.build())")
         for name, (res, args) in _SIGNATURES.items():
             fn = getattr(handle, name)
             fn.restype = res

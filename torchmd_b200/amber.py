@@ -24,6 +24,16 @@ semantics step by step:
   number, ``CMAP_PARAMETER_nn`` is read phi-major (psi fastest) from -180 deg, the way parmed
   reads it.  That ordering is restated from format documentation, not pinned against AMBER's
   own engine.
+* Urey-Bradley terms of chamber files, built only when asked for ``"ureybradley"``:
+  ``CHARMM_UREY_BRADLEY_COUNT`` (terms, types), ``CHARMM_UREY_BRADLEY`` rows (i, k, type) with
+  1-based atom indices, ``CHARMM_UREY_BRADLEY_FORCE_CONSTANT`` (kcal/mol/A^2, E = k (r - r0)^2)
+  and ``CHARMM_UREY_BRADLEY_EQUIL_VALUE`` (A).  Each term must join the ends of one of the
+  file's angles.  The layout follows parmed's ``ChamberParm``; it is not pinned against an engine.
+* ``"nbfix"``: LJ A/B over the type names from the full ``LENNARD_JONES_ACOEF/BCOEF`` through
+  ``NONBONDED_PARM_INDEX`` (``TopologyParameters(nbfix=...)`` with sigma = (A/B)^(1/6),
+  epsilon = B^2 / 4A per type pair), so that off-diagonal pair modifications (chamber NBFIX,
+  parmed's ``changeLJPair``) are kept; without it A/B are Lorentz-Berthelot mixes of the
+  diagonal.  Chamber files' ``LENNARD_JONES_14_ACOEF/BCOEF`` are not read.
 
 Pinned by ``tests/test_amber_reader.py`` against the reference's stored known answers for
 ``tests/data/prod_alanine_dipeptide_amber`` (``tests/test_torchmd.py:517,605``,
@@ -155,10 +165,27 @@ class AmberSystem:
                 raise ValueError(f"{prmtop_path}: CMAP_INDEX does not hold {nterm} terms on maps 1..{nmap}")
             self.cmap_idx, self.cmap_map = rows[:, :5], rows[:, 5]
 
+        # chamber Urey-Bradley: term (i, k) -> type; type -> (k_ub, s0)
+        self.ub_idx = np.zeros((0, 2), np.int64)
+        self.ub_type = np.zeros(0, np.int64)
+        self.ub_params = np.zeros((0, 2), np.float64)
+        if "CHARMM_UREY_BRADLEY_COUNT" in p:
+            nub, ntyp = p["CHARMM_UREY_BRADLEY_COUNT"][:2]
+            rows = _chunks(p["CHARMM_UREY_BRADLEY"], 3)[:nub] - 1
+            k, r0 = p["CHARMM_UREY_BRADLEY_FORCE_CONSTANT"][:ntyp], p["CHARMM_UREY_BRADLEY_EQUIL_VALUE"][:ntyp]
+            if len(rows) != nub or len(k) != ntyp or len(r0) != ntyp:
+                raise ValueError(f"{prmtop_path}: the Urey-Bradley sections do not hold {nub} terms of {ntyp} types")
+            if nub and (rows[:, :2].min() < 0 or rows[:, :2].max() >= self.natoms or rows[:, 2].min() < 0 or rows[:, 2].max() >= ntyp):
+                raise ValueError(f"{prmtop_path}: CHARMM_UREY_BRADLEY refers to an atom outside 1..{self.natoms} or a type outside 1..{ntyp}")
+            self.ub_idx, self.ub_type = rows[:, :2], rows[:, 2]
+            self.ub_params = np.stack([np.asarray(k, np.float64), np.asarray(r0, np.float64)], axis=1).reshape(-1, 2)
+
         # ---- per-type parameters, keyed by AMBER atom-type names like parmed's ParameterSet
         nb_idx = np.array(p["ATOM_TYPE_INDEX"], dtype=np.int64) - 1
         acoef, bcoef = p["LENNARD_JONES_ACOEF"], p["LENNARD_JONES_BCOEF"]
         nbparm = p["NONBONDED_PARM_INDEX"]
+        self._nb = (nb_idx, np.asarray(acoef, np.float64), np.asarray(bcoef, np.float64), np.asarray(nbparm, np.int64),
+                    np.asarray(p.get("HBOND_ACOEF", []), np.float64), np.asarray(p.get("HBOND_BCOEF", []), np.float64))
         rmin, depth = [], []
         for i in range(self.ntypes):  # parmed AmberParm.fill_LJ
             lj = nbparm[self.ntypes * i + i] - 1
@@ -207,6 +234,46 @@ class AmberSystem:
             elif first_quad[canon] in (tuple(q), tuple(q[::-1])):
                 self.dihedral_types[canon].append(term)
 
+    def nbfix_pairs(self, names):
+        """(pairs (P,2) into ``names``, (sigma, epsilon) (P,2)) for every pair a <= b of the type names, from the
+        full ACOEF/BCOEF tables.  A pair of a 10-12 hydrogen-bond term (negative index) with zero coefficients, as
+        TIP3P's HW-OW in many prmtops, has no LJ; one with a non-zero 10-12 term raises, and so do two atoms of one
+        name with different LJ rows."""
+        nb_idx, acoef, bcoef, nbparm, hba, hbb = self._nb
+        rows = {}
+        for i, t in enumerate(self.atomtype):
+            rows.setdefault(t, set()).add(int(nb_idx[i]))
+        used = sorted({int(x) for x in nb_idx})
+        entry = {}
+        for a in used:
+            for b in used:
+                e = int(nbparm[self.ntypes * a + b])
+                if e < 0 and (hba[-e - 1] != 0.0 or hbb[-e - 1] != 0.0):
+                    raise ValueError("the prmtop has 10-12 hydrogen-bond terms between the atoms' types: 'nbfix' cannot express them")
+                entry[(a, b)] = e - 1 if e > 0 else None
+        acoef, bcoef = np.append(acoef, 0.0), np.append(bcoef, 0.0)  # (index -1: a pair without LJ)
+        entry = {k: (len(acoef) - 1 if e is None else e) for k, e in entry.items()}
+        for t, ix in rows.items():
+            first = min(ix)
+            for o in ix:
+                if any(acoef[entry[(o, b)]] != acoef[entry[(first, b)]] or bcoef[entry[(o, b)]] != bcoef[entry[(first, b)]]
+                       for b in used):
+                    raise ValueError(f"atoms of type {t} have different Lennard-Jones rows in the prmtop")
+        pairs, prm = [], []
+        for a in range(len(names)):
+            for b in range(a, len(names)):
+                e = entry[(min(rows[names[a]]), min(rows[names[b]]))]
+                A, B = acoef[e], bcoef[e]
+                if A < 1.0e-10:
+                    sig, eps = 0.0, 0.0
+                elif B <= 0.0:
+                    raise ValueError(f"the LJ pair {names[a]}-{names[b]} is purely repulsive: 'nbfix' cannot express it")
+                else:
+                    sig, eps = (A / B) ** (1.0 / 6.0), B * B / (4.0 * A)
+                pairs.append([a, b])
+                prm.append([sig, eps])
+        return np.array(pairs, np.int64).reshape(-1, 2), np.array(prm, np.float64).reshape(-1, 2)
+
     # lookups with the reference's fall-backs (ff_parmed.py:81-129)
     def dihedral_terms(self, key):
         for var in (tuple(key), tuple(key)[::-1]):
@@ -226,7 +293,9 @@ class AmberSystem:
 def amber_parameters(system, terms=None, precision=torch.float32, device="cpu"):
     """``TopologyParameters`` for an ``AmberSystem`` -- the reference's
     ``Parameters(ParmedForcefield(mol, prmtop), mol, terms)`` (parameters.py:109-294).  ``"cmap"`` in ``terms``
-    (not among the defaults) also builds the file's CMAP terms; without it they are left out with a warning."""
+    (not among the defaults) also builds the file's CMAP terms, ``"ureybradley"`` a chamber file's Urey-Bradley
+    terms; without them they are left out with a warning.  ``"nbfix"`` takes the LJ tables from the file's full
+    ACOEF/BCOEF (module docstring)."""
     if terms is None:
         terms = ("bonds", "angles", "dihedrals", "impropers", "1-4", "lj")
     terms = [t.lower() for t in terms]
@@ -302,6 +371,21 @@ def amber_parameters(system, terms=None, precision=torch.float32, device="cpu"):
                     rows.append([ep * 4 * s6 * s6, ep * 4 * s6, term[3], term[4]])
                 pmap.append([i, row_of[key]])
             pairs14 = (d14[:, [0, 3]], np.array(pmap, dtype=np.int64), np.array(rows, dtype=np.float64))
+    urey_bradley = None
+    if len(system.ub_idx):
+        if "ureybradley" in terms:
+            angle_of = {(int(a), int(c)): i for i, (a, _, c) in enumerate(uqangles)}
+            rows = []
+            for a, c in system.ub_idx:
+                i = angle_of.get((min(int(a), int(c)), max(int(a), int(c))))
+                if i is None:
+                    raise ValueError(f"Urey-Bradley term {int(a) + 1}-{int(c) + 1} does not join the ends of an angle")
+                rows.append(i)
+            urey_bradley = (uqangles[rows], np.stack([np.arange(len(rows)), system.ub_type], 1), system.ub_params)
+        else:
+            warnings.warn(f"the topology has {len(system.ub_idx)} Urey-Bradley terms; they are left out unless terms includes "
+                          "'ureybradley'", stacklevel=2)
+    nbfix = system.nbfix_pairs(list(uq)) if "nbfix" in terms else None
     cmaps = None
     if len(system.cmap_idx):
         if "cmap" in terms:
@@ -321,6 +405,8 @@ def amber_parameters(system, terms=None, precision=torch.float32, device="cpu"):
         impropers=impropers,
         pairs14=pairs14,
         cmaps=cmaps,
+        urey_bradley=urey_bradley,
+        nbfix=nbfix,
         precision=precision,
         device=device,
     )

@@ -123,14 +123,21 @@ class CharmmPrmForceField:
     (torchmd/forcefields/forcefield.py:5-43), with the look-up semantics of its parmed adapter
     (ff_parmed.py:49-129), which this image cannot run (no parmed):
 
-    * bonds, angles: exact type tuple, either direction; Urey-Bradley columns are ignored (ff_parmed.py:73-75
-      returns only k, theta_eq);
+    * bonds, angles: exact type tuple, either direction; ``get_angle`` returns only k, theta_eq (ff_parmed.py:73-75);
+    * Urey-Bradley (not in the reference): columns 6-7 of an ANGLES line, k_ub [kcal/mol/A^2] and s0 [A], with
+      E = k_ub (r13 - s0)^2; ``get_urey_bradley`` gives them for a type triple in either direction, None when the
+      line has none;
     * dihedrals: exact type tuple or its reverse (ff_parmed.py:77-95, no wildcard matching there); lines that
       repeat a key add a term, a repeated periodicity replaces the earlier one (parmed's CharmmParameterSet);
     * 1-4: scnb = scee = 1 (parmed's default for CHARMM dihedral types) and the types' 1-4 sigma / epsilon -- the
       second column triple of a NONBONDED line when present, else the ordinary values (ff_parmed.py:97-113);
-    * LJ: epsilon = |eps|, sigma = (Rmin/2) * 2 * 2^(-1/6); NBFIX pairs are not used (the adapter reads only the
-      per-type values; the reference's own test notes "I don't have nbfix", tests/test_torchmd.py:326);
+    * LJ: epsilon = |eps|, sigma = (Rmin/2) * 2 * 2^(-1/6) (the adapter reads only the per-type values; the
+      reference's own test notes "I don't have nbfix", tests/test_torchmd.py:326);
+    * NBFIX (not in the reference): ``type1 type2 emin rmin [emin14 rmin14]`` with rmin = Rmin_ij itself, not a
+      half-radius: epsilon = |emin|, sigma = rmin * 2^(-1/6).  ``get_nbfix`` gives (sigma, epsilon, sigma14,
+      epsilon14) for a type pair in either order, None when there is no line; the 1-4 values are the 14 columns
+      when the line has them and the ordinary pair otherwise.  That 1-4 rule is restated from CHARMM's
+      parameter-file documentation, not checked against CHARMM itself;
     * impropers (harmonic, periodicity 0): parmed keys them by the SORTED type tuple; the adapter tries the
       permutations that keep position 2 (ff_parmed.py:115-129).  This part of parmed is restated from its
       documentation, not pinned: fixtures with impropers are labelled so in tests/golden.
@@ -145,6 +152,8 @@ class CharmmPrmForceField:
         self.mol = mol
         self.bonds, self.angles, self.dihedrals, self.impropers, self.lj, self.masses = {}, {}, {}, {}, {}, {}
         self.cmaps = {}  # 8 atom types -> (n, n) grid, phi-major
+        self.ub = {}  # 3 atom types (both directions) -> (k_ub, s0)
+        self.nbfix = {}  # 2 atom types (both orders) -> (sigma, epsilon, sigma14, epsilon14)
         cmap_key, cmap_vals, cmap_res = None, [], 0
         section, carry = None, ""
         for raw in open(path):
@@ -170,6 +179,8 @@ class CharmmPrmForceField:
                 elif section == "ANGLES":
                     a, b, c = (x.upper() for x in w[:3])
                     self.angles[(a, b, c)] = self.angles[(c, b, a)] = (float(w[3]), float(w[4]))
+                    if len(w) >= 7:
+                        self.ub[(a, b, c)] = self.ub[(c, b, a)] = (float(w[5]), float(w[6]))
                 elif section == "DIHEDRALS":
                     key = tuple(x.upper() for x in w[:4])
                     term = [float(w[4]), math.radians(float(w[6])), int(float(w[5]))]
@@ -187,6 +198,12 @@ class CharmmPrmForceField:
                     eps14, rmin14_half = (abs(float(w[5])), float(w[6])) if len(w) >= 7 else (eps, rmin_half)
                     f = 2.0 * 2.0 ** (-1.0 / 6.0)
                     self.lj[t] = (rmin_half * f, eps, rmin14_half * f, eps14)
+                elif section == "NBFIX":
+                    a, b = w[0].upper(), w[1].upper()
+                    f = 2.0 ** (-1.0 / 6.0)
+                    eps, sig = abs(float(w[2])), float(w[3]) * f
+                    eps14, sig14 = (abs(float(w[4])), float(w[5]) * f) if len(w) >= 6 else (eps, sig)
+                    self.nbfix[(a, b)] = self.nbfix[(b, a)] = (sig, eps, sig14, eps14)
                 elif section == "CMAP":
                     if cmap_key is None:  # header: 8 atom types and the resolution
                         cmap_res = int(w[8])
@@ -246,6 +263,14 @@ class CharmmPrmForceField:
         if key not in self.cmaps:
             raise RuntimeError(f"Could not find CMAP parameters for {key}")
         return self.cmaps[key]
+
+    def get_urey_bradley(self, at1, at2, at3):
+        """(k_ub, s0) of the angle type, either direction, or None when its line has no Urey-Bradley columns."""
+        return self.ub.get((str(at1).upper(), str(at2).upper(), str(at3).upper()))
+
+    def get_nbfix(self, at1, at2):
+        """(sigma, epsilon, sigma14, epsilon14) of the NBFIX line of the type pair, either order, or None."""
+        return self.nbfix.get((str(at1).upper(), str(at2).upper()))
 
     def get_improper(self, at1, at2, at3, at4):
         from itertools import permutations

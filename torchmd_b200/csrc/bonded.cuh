@@ -1,4 +1,4 @@
-// bonded.cuh -- bonded terms (K4): bonds, angles, proper/improper torsions, 1-4, CMAP correction maps.
+// bonded.cuh -- bonded terms (K4): bonds, angles, proper/improper torsions, 1-4, CMAP correction maps, Urey-Bradley.
 //
 // Replaces forces.py:122-258 (+ evaluate_bonds/angles/torsion, forces.py:494-605).
 //
@@ -20,8 +20,8 @@ namespace tmd {
 constexpr int BONDED_THREADS = 128;
 
 // kinds of term instance an atom entry can point at
-enum { BK_BOND = 0, BK_ANGLE = 1, BK_DIHEDRAL = 2, BK_IMPROPER = 3, BK_PAIR14 = 4, BK_CMAP = 5 };
-constexpr int BK_KINDS = 6;
+enum { BK_BOND = 0, BK_ANGLE = 1, BK_DIHEDRAL = 2, BK_IMPROPER = 3, BK_PAIR14 = 4, BK_CMAP = 5, BK_UREY_BRADLEY = 6 };
+constexpr int BK_KINDS = 7;
 
 // packed atom entry: kind (3 bits) | slot in the term (3 bits) | term index (26 bits)
 __host__ __device__ __forceinline__ unsigned bonded_entry(int kind, int slot, unsigned t) {
@@ -36,6 +36,7 @@ struct BondedTables {
   const int* entries;    // bonded_entry(kind, slot, term)
   BondedSet bonds, angles, torsions[2], pairs14;
   CmapSet cmap;
+  BondedSet ub;  // Urey-Bradley: idx (n,2) = the ends of an angle, prm (n,2) = k_ub, s0
 };
 
 struct BoxView {
@@ -113,17 +114,21 @@ __device__ __forceinline__ double cmap_term(const CmapSet& C, int t, const Vec3d
 
 __device__ __forceinline__ bool bonded_term(const DeviceState& S, const BondedTables& T, const float* __restrict__ q_scaled,
                                             const float* __restrict__ pos, size_t base, const BoxView& bx, int kind, int t, TermForces& o) {
-  if (kind == BK_BOND) {
-    // E = k (r-r0)^2; bonds longer than the cutoff are skipped like the reference (forces.py:128-136)
-    const int i = T.bonds.idx[2 * t], j = T.bonds.idx[2 * t + 1];
+  if (kind == BK_BOND || kind == BK_UREY_BRADLEY) {
+    // E = k (r-r0)^2.  Bonds longer than the cutoff are skipped like the reference (forces.py:128-136); Urey-Bradley
+    // terms (the ends of an angle, k_ub and s0) have no reference counterpart and are never cutoff-filtered.
+    const BondedSet& B = kind == BK_BOND ? T.bonds : T.ub;
+    const int i = B.idx[2 * t], j = B.idx[2 * t + 1];
     o.n = 2, o.atom[0] = i, o.atom[1] = j;
     const Vec3 pi = load3(pos, base + i), pj = load3(pos, base + j);
-    const Vec3 dref = delta_ref(pi, pj, bx.periodic, bx.L, bx.invL);
-    if (S.pp.has_cutoff && !(sqrt_rn(norm2_ref(dref.x, dref.y, dref.z)) <= S.pp.cutoff)) return false;  // reference decision
+    if (kind == BK_BOND && S.pp.has_cutoff) {
+      const Vec3 dref = delta_ref(pi, pj, bx.periodic, bx.L, bx.invL);
+      if (!(sqrt_rn(norm2_ref(dref.x, dref.y, dref.z)) <= S.pp.cutoff)) return false;  // reference decision
+    }
     const Vec3d d = delta_f64(pi, pj, bx.periodic, bx.L);
     const double dist = norm(d);
     double dedr;
-    bond_term<double>(dist, T.bonds.prm[2 * t], T.bonds.prm[2 * t + 1], o.e, dedr);
+    bond_term<double>(dist, B.prm[2 * t], B.prm[2 * t + 1], o.e, dedr);
     const Vec3d fv = (dedr / dist) * d;  // force on j; i gets the opposite
     o.f[0] = {-fv.x, -fv.y, -fv.z};
     o.f[1] = fv;
@@ -193,7 +198,7 @@ __device__ __forceinline__ bool bonded_term(const DeviceState& S, const BondedTa
 
 __device__ __forceinline__ void book_energy(BondedEnergies& E, int kind, const TermForces& o) {
   if (kind == BK_BOND) E.bond += o.e;
-  else if (kind == BK_ANGLE) E.angle += o.e;
+  else if (kind == BK_ANGLE || kind == BK_UREY_BRADLEY) E.angle += o.e;  // Urey-Bradley energy is booked as angle energy
   else if (kind == BK_DIHEDRAL || kind == BK_CMAP) E.dih += o.e;  // CMAP energy is booked as dihedral energy
   else if (kind == BK_IMPROPER) E.imp += o.e;
   else E.lj += o.e, E.el += o.e2;
@@ -219,7 +224,7 @@ __device__ __forceinline__ Vec3d bonded_force_on_atom(const DeviceState& S, cons
 
 // Where the force of (kind, term, slot) sits in the per-term buffer: slots of a kind side by side
 struct TermLayout {
-  int first[BK_KINDS];  // first term index (over all kinds, in the order bonds, angles, dihedrals, impropers, 1-4, CMAP) of each kind
+  int first[BK_KINDS];  // first term index (over all kinds, in the order of the BK_ enum) of each kind
   int slot0[BK_KINDS];  // first buffer slot of each kind
   int nterms, nslots;
 };
@@ -232,7 +237,7 @@ __device__ __forceinline__ void bonded_energy_reduce(const DeviceState& S, const
                                                      double* __restrict__ energies, double* red) {
   double* Eo = energies + (size_t)r * TMD_NUM_ENERGIES;
   if (T.bonds.n) block_accumulate<BONDED_THREADS / 32>(E.bond, Eo + TMD_E_BONDS, red);
-  if (T.angles.n) block_accumulate<BONDED_THREADS / 32>(E.angle, Eo + TMD_E_ANGLES, red);
+  if (T.angles.n || T.ub.n) block_accumulate<BONDED_THREADS / 32>(E.angle, Eo + TMD_E_ANGLES, red);
   if (T.torsions[0].n || T.cmap.n) block_accumulate<BONDED_THREADS / 32>(E.dih, Eo + TMD_E_DIHEDRALS, red);
   if (T.torsions[1].n) block_accumulate<BONDED_THREADS / 32>(E.imp, Eo + TMD_E_IMPROPERS, red);
   if (T.pairs14.n) {
@@ -249,7 +254,7 @@ k_bonded_terms(DeviceState S, BondedTables T, TermLayout lay, const float* __res
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
   BondedEnergies E;
   if (g < lay.nterms) {
-    int kind = BK_CMAP;
+    int kind = BK_KINDS - 1;
 #pragma unroll
     for (int k = BK_KINDS - 2; k >= 0; --k)
       if (g < lay.first[k + 1]) kind = k;

@@ -177,6 +177,8 @@ struct tmd_ctx {
   std::vector<int32_t> bonds_idx_h, angles_idx_h, torsions_idx_h[2], pairs14_idx_h;  // host copies for the atom CSR
   tmd::CmapSet cmap;                 // CMAP terms and maps (tmd_set_cmap), both precisions
   std::vector<int32_t> cmap_idx_h;
+  tmd::BondedSet ub;                 // Urey-Bradley 1-3 terms (tmd_set_urey_bradley): idx (n,2), prm (n,2) = k_ub, s0
+  std::vector<int32_t> ub_idx_h;
   int* bonded_atom_ptr = nullptr;    // device CSR: atom -> bonded term entries (see bonded.cuh)
   int* bonded_entries = nullptr;
   int bonded_nentries = 0;
@@ -219,5 +221,5 @@ struct tmd_ctx {
   double* AB64 = nullptr;
   double* L64 = nullptr;
   std::vector<double> charges64_host, box64_host;
-  tmd::BondedSetT<double> bonds64, angles64, torsions64[2], pairs1464;
+  tmd::BondedSetT<double> bonds64, angles64, torsions64[2], pairs1464, ub64;
 };

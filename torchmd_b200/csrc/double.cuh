@@ -249,6 +249,7 @@ struct BondedTables64 {
   const int* entries;
   BondedSetT<double> bonds, angles, torsions[2], pairs14;
   CmapSet cmap;
+  BondedSetT<double> ub;
 };
 
 __device__ __forceinline__ Vec3d load3d(const double* p, size_t atom) {
@@ -270,14 +271,15 @@ __device__ __forceinline__ bool bonded_term_f64(const DeviceState& S, const Devi
   const size_t base = (size_t)r * S.natoms;
   const int periodic = S.grid[r].periodic;
   const double* L = D.L + 3 * r;
-  if (kind == BK_BOND) {
-    const int i = T.bonds.idx[2 * t], j = T.bonds.idx[2 * t + 1];
+  if (kind == BK_BOND || kind == BK_UREY_BRADLEY) {  // Urey-Bradley: k_ub (r13 - s0)^2, no cutoff filter (bonded.cuh)
+    const BondedSetT<double>& B = kind == BK_BOND ? T.bonds : T.ub;
+    const int i = B.idx[2 * t], j = B.idx[2 * t + 1];
     o.n = 2, o.atom[0] = i, o.atom[1] = j;
     const Vec3d d = delta64(load3d(pos, base + i), load3d(pos, base + j), periodic, L);
     const double dist = sqrt_rn(norm2_ref(d.x, d.y, d.z));
-    if (D.pp.has_cutoff && !(dist <= D.pp.cutoff)) return false;  // forces.py:128-136, the fp64 decision
+    if (kind == BK_BOND && D.pp.has_cutoff && !(dist <= D.pp.cutoff)) return false;  // forces.py:128-136, the fp64 decision
     double dedr;
-    bond_term<double>(dist, T.bonds.prm[2 * t], T.bonds.prm[2 * t + 1], o.e, dedr);
+    bond_term<double>(dist, B.prm[2 * t], B.prm[2 * t + 1], o.e, dedr);
     const Vec3d fv = (dedr / dist) * d;
     o.f[0] = {-fv.x, -fv.y, -fv.z};
     o.f[1] = fv;
@@ -346,7 +348,7 @@ __device__ __forceinline__ void bonded_energy_reduce64(const DeviceState64& D, c
                                                        const BondedEnergies& E, double* __restrict__ energies, double* red) {
   double* Eo = energies + (size_t)r * TMD_NUM_ENERGIES;
   if (T.bonds.n) block_accumulate<BONDED_THREADS / 32>(E.bond, Eo + TMD_E_BONDS, red);
-  if (T.angles.n) block_accumulate<BONDED_THREADS / 32>(E.angle, Eo + TMD_E_ANGLES, red);
+  if (T.angles.n || T.ub.n) block_accumulate<BONDED_THREADS / 32>(E.angle, Eo + TMD_E_ANGLES, red);
   if (T.torsions[0].n || T.cmap.n) block_accumulate<BONDED_THREADS / 32>(E.dih, Eo + TMD_E_DIHEDRALS, red);
   if (T.torsions[1].n) block_accumulate<BONDED_THREADS / 32>(E.imp, Eo + TMD_E_IMPROPERS, red);
   if (T.pairs14.n) {
@@ -362,7 +364,7 @@ k_bonded_terms_f64(DeviceState S, DeviceState64 D, BondedTables64 T, TermLayout 
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
   BondedEnergies E;
   if (g < lay.nterms) {
-    int kind = BK_CMAP;
+    int kind = BK_KINDS - 1;
 #pragma unroll
     for (int k = BK_KINDS - 2; k >= 0; --k)
       if (g < lay.first[k + 1]) kind = k;

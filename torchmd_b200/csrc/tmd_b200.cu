@@ -332,7 +332,7 @@ const char* tmd_last_error(void) { return g_err.c_str(); }
 #if defined(TMD_SIMT_HOST)
 int tmd_version(void) { return -100; }  // host SIMT interpreter build (tests/simt): torchmd_b200/_lib.py refuses it
 #else
-int tmd_version(void) { return 105; }  // 101: the "precision: double" entry points (tmd_set_precision, *_f64); 102: constraints; 103: PME; 104: box rescale + molecule scaling; 105: CMAP
+int tmd_version(void) { return 106; }  // 101: the "precision: double" entry points (tmd_set_precision, *_f64); 102: constraints; 103: PME; 104: box rescale + molecule scaling; 105: CMAP; 106: Urey-Bradley
 #endif
 
 int tmd_create(tmd_ctx** out, int device, int natoms, int nreplicas) {
@@ -396,7 +396,8 @@ int tmd_destroy(tmd_ctx* ctx) {
                   ctx->bonds64.idx, ctx->bonds64.prm, ctx->angles64.idx, ctx->angles64.prm,
                   ctx->torsions64[0].idx, ctx->torsions64[0].term_ptr, ctx->torsions64[0].terms,
                   ctx->torsions64[1].idx, ctx->torsions64[1].term_ptr, ctx->torsions64[1].terms,
-                  ctx->pairs1464.idx, ctx->pairs1464.prm, ctx->cmap.idx, ctx->cmap.map_of, ctx->cmap.maps, ctx->cmap.coef};
+                  ctx->pairs1464.idx, ctx->pairs1464.prm, ctx->cmap.idx, ctx->cmap.map_of, ctx->cmap.maps, ctx->cmap.coef,
+                  ctx->ub.idx, ctx->ub.prm, ctx->ub64.idx, ctx->ub64.prm};
   for (void* b : bufs)
     if (b) cudaFree(b);
   dd_release(ctx);
@@ -573,6 +574,27 @@ int tmd_set_pairs14(tmd_ctx* ctx, int n, const int32_t* idx, const float* prm) {
   if (!ctx) return fail(TMD_ERR_ARG, "null context");
   TMD_PRECISION(ctx, 32, "tmd_set_pairs14")
   return set_bonded(ctx, ctx->pairs14, ctx->pairs14_idx_h, n, 2, 4, idx, prm);
+}
+extern "C++" {  // (templates inside the C-linkage block)
+// Urey-Bradley terms: two distinct atoms each, k_ub finite and >= 0, s0 finite; then stored like bonds.
+template <typename P>
+static int set_urey_bradley(tmd_ctx* ctx, BondedSetT<P>& s, int n, const int32_t* idx, const P* prm) {
+  if (n < 0 || (n > 0 && (!idx || !prm))) return fail(TMD_ERR_ARG, "tmd_set_urey_bradley: bad arguments");
+  for (long long e = 0; e < (long long)n * 2; ++e)
+    if (idx[e] < 0 || idx[e] >= ctx->natoms) return fail(TMD_ERR_ARG, "tmd_set_urey_bradley: atom index out of range");
+  for (int t = 0; t < n; ++t) {
+    if (idx[2 * t] == idx[2 * t + 1]) return fail(TMD_ERR_ARG, "tmd_set_urey_bradley: a term joins an atom to itself");
+    if (!std::isfinite((double)prm[2 * t]) || prm[2 * t] < 0)
+      return fail(TMD_ERR_ARG, "tmd_set_urey_bradley: force constant negative or not finite");
+    if (!std::isfinite((double)prm[2 * t + 1])) return fail(TMD_ERR_ARG, "tmd_set_urey_bradley: distance not finite");
+  }
+  return set_bonded(ctx, s, ctx->ub_idx_h, n, 2, 2, idx, prm);
+}
+}  // extern "C++"
+int tmd_set_urey_bradley(tmd_ctx* ctx, int n, const int32_t* idx, const float* prm) {
+  if (!ctx) return fail(TMD_ERR_ARG, "null context");
+  TMD_PRECISION(ctx, 32, "tmd_set_urey_bradley")
+  return set_urey_bradley(ctx, ctx->ub, n, idx, prm);
 }
 extern "C++" {  // (templates inside the C-linkage block)
 template <typename P>
@@ -758,6 +780,11 @@ int tmd_set_pairs14_f64(tmd_ctx* ctx, int n, const int32_t* idx, const double* p
   if (!ctx) return fail(TMD_ERR_ARG, "null context");
   TMD_PRECISION(ctx, 64, "tmd_set_pairs14_f64")
   return set_bonded(ctx, ctx->pairs1464, ctx->pairs14_idx_h, n, 2, 4, idx, prm);
+}
+int tmd_set_urey_bradley_f64(tmd_ctx* ctx, int n, const int32_t* idx, const double* prm) {
+  if (!ctx) return fail(TMD_ERR_ARG, "null context");
+  TMD_PRECISION(ctx, 64, "tmd_set_urey_bradley_f64")
+  return set_urey_bradley(ctx, ctx->ub64, n, idx, prm);
 }
 int tmd_set_torsions_f64(tmd_ctx* ctx, int which, int n, const int32_t* idx, const int32_t* term_ptr,
                          const double* terms, int amber_form) {
@@ -1325,13 +1352,14 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   {
     const uint32_t bm = ctx->bonded_mask;
     struct Src { int kind, k; const std::vector<int32_t>* idx; bool on; };
-    const Src src[6] = {
+    const Src src[7] = {
         {BK_BOND, 2, &ctx->bonds_idx_h, (bm & TMD_TERM(TMD_E_BONDS)) != 0},
         {BK_ANGLE, 3, &ctx->angles_idx_h, (bm & TMD_TERM(TMD_E_ANGLES)) != 0},
         {BK_DIHEDRAL, 4, &ctx->torsions_idx_h[0], (bm & TMD_TERM(TMD_E_DIHEDRALS)) != 0},
         {BK_PAIR14, 2, &ctx->pairs14_idx_h, (bm & TMD_TERM(TMD_E_14)) != 0},
         {BK_IMPROPER, 4, &ctx->torsions_idx_h[1], (bm & TMD_TERM(TMD_E_IMPROPERS)) != 0},
-        {BK_CMAP, 5, &ctx->cmap_idx_h, (bm & TMD_TERM(TMD_E_DIHEDRALS)) != 0}};  // CMAP acts with the dihedrals
+        {BK_CMAP, 5, &ctx->cmap_idx_h, (bm & TMD_TERM(TMD_E_DIHEDRALS)) != 0},  // CMAP acts with the dihedrals
+        {BK_UREY_BRADLEY, 2, &ctx->ub_idx_h, (bm & TMD_TERM(TMD_E_ANGLES)) != 0}};  // Urey-Bradley with the angles
     std::vector<int> ptr(N + 1, 0);
     for (const Src& sc : src)
       if (sc.on)
@@ -1515,7 +1543,8 @@ static inline dim3 owned_grid(const tmd_ctx* ctx, int threads) {
 
 // The kernels' bonded table (BondedTables or BondedTables64) from the context's sets, disabled terms emptied.
 template <typename Tables, typename Set>
-static Tables bonded_tables(const tmd_ctx* ctx, const Set& bonds, const Set& angles, const Set* torsions, const Set& pairs14) {
+static Tables bonded_tables(const tmd_ctx* ctx, const Set& bonds, const Set& angles, const Set* torsions, const Set& pairs14,
+                            const Set& ub) {
   const uint32_t bm = ctx->bonded_mask;
   Tables T;
   T.atom_ptr = ctx->bonded_atom_ptr;
@@ -1526,8 +1555,9 @@ static Tables bonded_tables(const tmd_ctx* ctx, const Set& bonds, const Set& ang
   T.torsions[1] = torsions[1];
   T.pairs14 = pairs14;
   T.cmap = ctx->cmap;
+  T.ub = ub;
   if (!(bm & TMD_TERM(TMD_E_BONDS))) T.bonds.n = 0;
-  if (!(bm & TMD_TERM(TMD_E_ANGLES))) T.angles.n = 0;
+  if (!(bm & TMD_TERM(TMD_E_ANGLES))) T.angles.n = 0, T.ub.n = 0;
   if (!(bm & TMD_TERM(TMD_E_DIHEDRALS))) T.torsions[0].n = 0, T.cmap.n = 0;
   if (!(bm & TMD_TERM(TMD_E_IMPROPERS))) T.torsions[1].n = 0;
   if (!(bm & TMD_TERM(TMD_E_14))) T.pairs14.n = 0;
@@ -1537,7 +1567,7 @@ static Tables bonded_tables(const tmd_ctx* ctx, const Set& bonds, const Set& ang
 template <typename Tables>
 static TermLayout term_layout(const Tables& T) {
   TermLayout lay;
-  const int cnt[BK_KINDS] = {T.bonds.n, T.angles.n, T.torsions[0].n, T.torsions[1].n, T.pairs14.n, T.cmap.n};
+  const int cnt[BK_KINDS] = {T.bonds.n, T.angles.n, T.torsions[0].n, T.torsions[1].n, T.pairs14.n, T.cmap.n, T.ub.n};
   int nt = 0, ns = 0;
   for (int k = 0; k < BK_KINDS; ++k) {
     lay.first[k] = nt;
@@ -1649,7 +1679,7 @@ static int enqueue_forces_f64(tmd_ctx* ctx, const double* pos, double* forces, d
     TMD_CUDA(cudaMemsetAsync(forces, 0, (size_t)R * N * 3 * sizeof(double), st));
   }
   if (ctx->bonded_nentries > 0) {
-    const BondedTables64 T = bonded_tables<BondedTables64>(ctx, ctx->bonds64, ctx->angles64, ctx->torsions64, ctx->pairs1464);
+    const BondedTables64 T = bonded_tables<BondedTables64>(ctx, ctx->bonds64, ctx->angles64, ctx->torsions64, ctx->pairs1464, ctx->ub64);
     const TermLayout lay = term_layout(T);
     launch(k_bonded_terms_f64, dim3((std::max(lay.nterms, 1) + BONDED_THREADS - 1) / BONDED_THREADS, R), BONDED_THREADS, st, d, D, T, lay,
            pos, energies, priv(ctx).term_forces);
@@ -1678,7 +1708,7 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
 
   BondedTables T;
   const bool have_bonded = ctx->bonded_nentries > 0;
-  if (have_bonded) T = bonded_tables<BondedTables>(ctx, ctx->bonds, ctx->angles, ctx->torsions, ctx->pairs14);
+  if (have_bonded) T = bonded_tables<BondedTables>(ctx, ctx->bonds, ctx->angles, ctx->torsions, ctx->pairs14, ctx->ub);
   // bonded forces of the owned atoms: terms in parallel, then the fixed-order sum per atom (bonded.cuh)
   auto launch_bonded = [&](cudaStream_t bs, double* scratch) -> int {
     CtxPriv& pv = priv(ctx);

@@ -108,7 +108,15 @@ def yaml_parameters(mol, forcefield, terms=None, precision=torch.float32, device
     ``"cmap"`` in ``terms`` (not among the defaults) builds CMAP terms from the molecule's ``crossterms`` (C,8) with a
     force field that has ``get_cmap`` (charmm.CharmmPrmForceField); without it they are left out with a warning.  A
     cross-term must be two dihedrals that share three atoms, (a,b,c,d) and (b,c,d,e), as every backbone phi/psi pair
-    is; it becomes the 5-atom term (a,b,c,d,e).  The grids keep the file's values (fp64)."""
+    is; it becomes the 5-atom term (a,b,c,d,e).  The grids keep the file's values (fp64).
+
+    ``"ureybradley"`` (not among the defaults) builds one Urey-Bradley term per unique angle whose type has k_ub > 0,
+    from a force field with ``get_urey_bradley`` (charmm.CharmmPrmForceField); ``"nbfix"`` (not among the defaults)
+    passes the force field's NBFIX pairs of the molecule's types to ``TopologyParameters(nbfix=...)``, and a 1-4 pair
+    whose two types have an NBFIX line takes that line's 1-4 sigma / epsilon instead of the Lorentz-Berthelot mix
+    (charmm.CharmmPrmForceField documents the 1-4 rule).  Without ``"ureybradley"``, Urey-Bradley terms the file has for
+    this molecule are left out with a warning; without ``"nbfix"`` the tables are the Lorentz-Berthelot ones, silently,
+    as they were before NBFIX was read.  A force field without those look-ups raises when the term is asked for."""
     # a force-field object with the reference's interface (YamlForceField, charmm.CharmmPrmForceField), or a YAML path / dict
     ff = forcefield if hasattr(forcefield, "get_LJ") else YamlForceField(forcefield)
     if terms is None:
@@ -149,7 +157,36 @@ def yaml_parameters(mol, forcefield, terms=None, precision=torch.float32, device
     uqbonds = np.unique(np.sort(bonds_raw, axis=1), axis=0) if len(bonds_raw) else bonds_raw
     uqangles = oriented(angles_raw) if len(angles_raw) else angles_raw
     uqdih = oriented(dih_raw) if len(dih_raw) else dih_raw
-    bonds = angles = dihedrals = impropers = pairs14 = None
+    bonds = angles = dihedrals = impropers = pairs14 = urey_bradley = nbfix = None
+    for term, lookup in (("ureybradley", "get_urey_bradley"), ("nbfix", "get_nbfix")):
+        if term in terms and not hasattr(ff, lookup):
+            raise RuntimeError(f"'{term}' was asked for, but the force field has no {term} parameters")
+    fix = {}  # (type index, type index) -> (sigma, epsilon, sigma14, epsilon14)
+    if hasattr(ff, "get_nbfix"):
+        for a in range(len(uq)):
+            for b in range(a, len(uq)):
+                v = ff.get_nbfix(uq[a], uq[b])
+                if v is not None:
+                    fix[(a, b)] = v
+    if fix and "nbfix" in terms:
+        nbfix = (np.array(list(fix), np.int64), _f32([[v[0], v[1]] for v in fix.values()]))
+    if hasattr(ff, "get_urey_bradley") and len(uqangles):
+        rows, row_of, pmap, keep = [], {}, [], []
+        for i, atoms in enumerate(uqangles):
+            key = tuple(T[atoms])
+            ub = ff.get_urey_bradley(*key)
+            if ub is None or not ub[0] > 0:
+                continue
+            if key not in row_of:
+                row_of[key] = len(rows)
+                rows.append(list(ub))
+            pmap.append([len(keep), row_of[key]])
+            keep.append(i)
+        if keep and "ureybradley" not in terms:
+            warnings.warn(f"the molecule has {len(keep)} angles with a Urey-Bradley term; they are left out unless terms "
+                          "includes 'ureybradley'", stacklevel=2)
+        elif keep:
+            urey_bradley = (uqangles[keep], np.array(pmap, np.int64), _f32(rows))
     if "bonds" in terms and len(uqbonds):
         bonds = typed(uqbonds, ff.get_bond)
     if "angles" in terms and len(uqangles):
@@ -197,6 +234,9 @@ def yaml_parameters(mol, forcefield, terms=None, precision=torch.float32, device
                 key = tuple(T[atoms])
                 scnb, scee, s1, e1, s4, e4 = ff.get_14(*key)
                 sig, ep = 0.5 * (s1 + s4), math.sqrt(e1 * e4)
+                fx = ff.get_nbfix(key[0], key[3]) if nbfix is not None else None
+                if fx is not None:
+                    sig, ep = fx[2], fx[3]
                 s6 = sig**6
                 if key[::-1] in row_of:
                     key = key[::-1]
@@ -236,6 +276,8 @@ def yaml_parameters(mol, forcefield, terms=None, precision=torch.float32, device
         impropers=impropers,
         pairs14=pairs14,
         cmaps=cmaps,
+        urey_bradley=urey_bradley,
+        nbfix=nbfix,
         precision=precision,
         device=device,
     )

@@ -58,7 +58,9 @@ class Forces:
     parameters : object with the reference ``Parameters`` attribute layout
     terms : list of str, case-insensitive, from ``Forces.terms``.  ``"dihedrals"`` also turns on the CMAP
         correction maps the parameters carry (``cmap_params``, built by the parameter builders when asked for
-        ``"cmap"``); their energy is part of the ``dihedrals`` energy.
+        ``"cmap"``); their energy is part of the ``dihedrals`` energy.  ``"angles"`` likewise turns on the Urey-Bradley
+        1-3 terms the parameters carry (``ub_params``, built when asked for ``"ureybradley"``); their energy is part of
+        the ``angles`` energy.
     external : optional plugin exposing ``calculate(pos, box) -> (E (R,), F (R,N,3))``
     cutoff, rfa, solventDielectric, switch_dist, exclusions : as in the reference
     skin : Verlet-list buffer in Angstrom (not in the reference; results do not depend on it)
@@ -284,6 +286,11 @@ class Forces:
             res, grids = _np(cmap["res"], np.int32), _np(cmap["grids"], np.float64)
             idx, map_of = _np(cmap["idx"], np.int32), _np(cmap["map_of"], np.int32)
             check(L.tmd_set_cmap(ctx, len(res), _lib.ptr(res), _lib.ptr(grids), len(idx), _lib.ptr(idx), _lib.ptr(map_of)))
+        ub = getattr(par, "ub_params", None)  # (a reference Parameters object has none)
+        if "angles" in self.energies and ub is not None and len(ub["idx"]):
+            idx, _, prm = instance_rows(ub)
+            ends = np.ascontiguousarray(idx[:, [0, 2]])
+            check(setter("tmd_set_urey_bradley")(ctx, len(ends), _lib.ptr(ends), _lib.ptr(prm)))
 
     def _ensure_box(self, box):
         """Hand the box diagonal to the context when the tensor changed (one D2H copy).  The tensor the

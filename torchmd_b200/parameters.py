@@ -16,6 +16,13 @@ CMAP correction maps (not in the reference) are ``cmap_params = {"idx": (n,5) in
 "res": (nmaps,) int64, "grids": (sum res^2,) float64}``: term t acts on atoms idx[t] with phi = dihedral(idx[t,0:4]),
 psi = dihedral(idx[t,1:5]) and map map_of[t]; map m holds E(phi_i, psi_j) at phi_i = -180 deg + i 360 deg / res[m]
 (psi alike), phi-major, in kcal/mol.  The grids stay fp64 in both precisions.
+
+Urey-Bradley terms (not in the reference) are ``ub_params`` in the per-term layout with idx (U,3) = the angle
+(a, b, c) whose ends a, c the term joins and params (P,2) = k_ub [kcal/mol/A^2], s0 [A]; E = k_ub (r_ac - s0)^2.
+
+NBFIX pair overrides (not in the reference) are ``nbfix_params = {"idx": (P,2) int64 type pairs, "params": (P,2)
+sigma, epsilon}``: ``get_AB`` puts 4 eps sigma^12 and 4 eps sigma^6 at (t1, t2) and (t2, t1) of the Lorentz-Berthelot
+tables and leaves every other entry as it was.
 """
 import numpy as np
 import torch
@@ -43,6 +50,16 @@ def _term(idx, pmap, params, dtype):
     pmap = torch.as_tensor(np.asarray(pmap), dtype=torch.int64)
     params = torch.as_tensor(np.asarray(params, dtype=np.float64)).to(dtype)
     return {"idx": idx, "map": pmap, "params": params}
+
+
+def _nbfix(pairs, params, ntypes):
+    pairs = torch.as_tensor(np.asarray(pairs, dtype=np.int64).reshape(-1, 2))
+    params = torch.as_tensor(np.asarray(params, dtype=np.float64).reshape(-1, 2))
+    if len(pairs) != len(params):
+        raise ValueError("nbfix: one (sigma, epsilon) row per type pair")
+    if len(pairs) and (int(pairs.min()) < 0 or int(pairs.max()) >= ntypes):
+        raise ValueError(f"nbfix: type index outside 0..{ntypes - 1}")
+    return {"idx": pairs, "params": params}
 
 
 def _cmap(idx, map_of, res, grids, natoms):
@@ -77,6 +94,8 @@ class TopologyParameters:
         impropers=None,
         pairs14=None,
         cmaps=None,
+        urey_bradley=None,
+        nbfix=None,
         precision=torch.float32,
         device="cpu",
     ):
@@ -87,6 +106,8 @@ class TopologyParameters:
         bonds/angles/dihedrals/impropers/pairs14 : optional ``(idx, map, params)``
             triples in the layout described in the module docstring.
         cmaps : optional ``(idx (n,5), map_of (n,), res (nmaps,), grids)`` CMAP terms and maps (module docstring)
+        urey_bradley : optional ``(idx (U,3) angle triples, map, params (P,2) = k_ub, s0)`` (module docstring)
+        nbfix : optional ``(type pairs (P,2), params (P,2) = sigma, epsilon)`` LJ overrides applied by ``get_AB``
         """
         self.natoms = int(len(atom_types))
         self.mapped_atom_types = torch.as_tensor(
@@ -111,6 +132,10 @@ class TopologyParameters:
         self.improper_params = _term(*impropers, torch.float64) if impropers else None
         self.nonbonded_14_params = _term(*pairs14, torch.float64) if pairs14 else None
         self.cmap_params = _cmap(*cmaps, self.natoms) if cmaps is not None and len(cmaps[0]) else None
+        self.ub_params = _term(*urey_bradley, torch.float64) if urey_bradley else None
+        if self.ub_params is not None and (int(self.ub_params["idx"].min()) < 0 or int(self.ub_params["idx"].max()) >= self.natoms):
+            raise ValueError("urey_bradley: atom index out of range")
+        self.nbfix_params = _nbfix(*nbfix, len(nb)) if nbfix is not None and len(nbfix[0]) else None
         self.A = None
         self.B = None
         self.device = "cpu"
@@ -126,6 +151,8 @@ class TopologyParameters:
             self.dihedral_params,
             self.improper_params,
             self.nonbonded_14_params,
+            self.ub_params,
+            self.nbfix_params,
         ]
 
     def to_(self, device):
@@ -151,7 +178,15 @@ class TopologyParameters:
 
     def get_AB(self):
         p = self.nonbonded_params["params"]
-        return lorentz_berthelot_AB(p[:, 0], p[:, 1])
+        A, B = lorentz_berthelot_AB(p[:, 0], p[:, 1])
+        if self.nbfix_params is not None:
+            ij = self.nbfix_params["idx"].to(A.device)
+            q = self.nbfix_params["params"].to(A.dtype).to(A.device)
+            s6 = q[:, 0] ** 6  # the operation order of lorentz_berthelot_AB
+            b, a = q[:, 1] * 4 * s6, q[:, 1] * 4 * s6 * s6
+            for i, j in ((ij[:, 0], ij[:, 1]), (ij[:, 1], ij[:, 0])):
+                A[i, j], B[i, j] = a, b
+        return A, B
 
     def get_exclusions(self, types=("bonds", "angles", "1-4"), fullarray=False):
         """Excluded pair list: bonded pairs, angle ends, dihedral ends
