@@ -105,6 +105,16 @@ inline void launch_smem(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t 
 #endif
 }
 
+// f(a, b) with a and b as std::integral_constant<bool, ...>: one launch line for the four <bool, bool> instantiations
+// of a kernel, as in with_bools(thermo, ke != nullptr, [&](auto th, auto e) { launch(k_vv_second<th, e>, ...); })
+template <typename F>
+inline void with_bools(bool a, bool b, F&& f) {
+  using T = std::true_type;
+  using N = std::false_type;
+  if (a) b ? f(T{}, T{}) : f(T{}, N{});
+  else b ? f(N{}, T{}) : f(N{}, N{});
+}
+
 struct DeviceGuard {
   int prev = -1;
   explicit DeviceGuard(int dev) {
@@ -159,6 +169,15 @@ static void stage_free(void* p) {
 }
 
 
+// The arguments of a tmd_md_steps call that every step reads (enqueue_step), and that a captured step bakes in.
+struct StepArgs {
+  float *pos, *vel, *forces;
+  const float *masses, *vcoeff;
+  double dt, gamma;
+  uint64_t seed, first_step;
+  double *energies, *ke;
+};
+
 struct CtxPriv {
   // TMD_B200_OVERLAP=1: bonded kernel on a second stream, concurrent with the pair kernel
   cudaStream_t side = nullptr;
@@ -178,13 +197,7 @@ struct CtxPriv {
   static constexpr int NGRAPH = 5;
   cudaGraphExec_t exec[NGRAPH] = {nullptr, nullptr, nullptr, nullptr, nullptr};
   cudaGraph_t graph[NGRAPH] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  struct StepKey {
-    float *pos, *vel, *forces;
-    const float *masses, *vcoeff;
-    double dt, gamma;
-    uint64_t seed, first_step;
-    double *energies, *ke;
-  } step_key{};
+  StepArgs step_key{};               // the arguments the captured steps were made for
   DeviceState step_state{};          // the kernel arguments baked into the captured steps
   bool steps_valid = false;
   int64_t step_launches[5] = {0, 0, 0, 0, 0};  // kernels of one captured step (rebuild body included)
@@ -195,19 +208,9 @@ struct CtxPriv {
   size_t term_forces_len = 0;
   bool flags_live = false;  // the device flags hold counts of this context (set by the first finalisation)
   bool fuse_step = false;   // TMD_B200_FUSESTEP=1: k_cstep_boundary between the steps of one tmd_md_steps call
-  bool fold_next = false;                       // tmd_md_steps: the vv_second that follows folds the bonded sums in (k_vv_second_fold)
-  bool fold_pending = false;                    // set by enqueue_forces when it left them in the scratch buffer
-  bool prepared = false;                        // the next enqueue_forces finds k_prepare's work done
-  cudaGraphConditionalHandle prepared_cond = 0; // and this handle already handed to the kernel
   bool dirty = true;
   size_t nbr_entries = 0;
-  // cluster path inside tmd_md_steps: the bonded kernel is folded into the second half-kick (fused.cuh)
   int64_t last_body_launches = 0; // kernels the last captured force call put into the rebuild's conditional body
-  bool defer_bonded = false;      // set by tmd_md_steps for the force call it is about to make
-  bool bonded_deferred = false;   // enqueue_forces left the bonded terms (and the unsort) to enqueue_vv_second
-  double* deferred_energies = nullptr;
-  BondedTables deferred_tables{};
-  const float* deferred_pos = nullptr;
   // cluster path: owned buffers behind ctx->d.cl
   std::vector<void*> cl_bufs;
   int cl_blocks = 0;        // CTAs of k_cpair per replica
@@ -1690,7 +1693,44 @@ static int enqueue_forces_f64(tmd_ctx* ctx, const double* pos, double* forces, d
   return TMD_OK;
 }
 
-static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double* energies, cudaStream_t st) {
+// What the kernels of one tmd_md_steps step hand each other (enqueue_step).  A standalone call passes no link: its
+// force call runs k_prepare and finishes its own forces, and its second half-kick is plain k_vv_second.
+struct StepLink {
+  bool prepared = false;                // in: the kernel before the force call did k_prepare's work,
+  cudaGraphConditionalHandle cond = 0;  // and switches the rebuild's conditional node with this handle (when capturing)
+  enum Tail { NONE, FOLD, DEFERRED } tail = NONE;  // out: what the force call left to the kernel after it
+  BondedTables T;                       // DEFERRED: k_bonded_vv_second evaluates these terms,
+  const float* pos = nullptr;           // at these positions,
+  double* energies = nullptr;           // and books their energies here
+};
+
+// The graph st is being captured into (TMD_B200_GRAPH), or nullptr.
+static cudaGraph_t capture_graph(tmd_ctx* ctx, cudaStream_t st) {
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  cudaGraph_t g = nullptr;
+  if (!priv(ctx).use_graph || cudaStreamGetCaptureInfo(st, &cs, nullptr, &g, nullptr, nullptr) != cudaSuccess ||
+      cs != cudaStreamCaptureStatusActive)
+    return nullptr;
+  return g;
+}
+// While st is being captured, the list rebuild of the force call becomes the body of a conditional node: make its
+// handle and give it to dp, the device state of the kernel that switches it on.  Not capturing: dp is left as it is.
+static int capture_cond(tmd_ctx* ctx, cudaStream_t st, DeviceState& dp) {
+  if (cudaGraph_t g = capture_graph(ctx, st)) {
+    cudaGraphConditionalHandle h = 0;
+    TMD_CUDA(cudaGraphConditionalHandleCreate(&h, g, 0, cudaGraphCondAssignDefault));
+    dp.cond = (unsigned long long)h;
+  }
+  return TMD_OK;
+}
+// TMD_B200_FUSEPREP, whole system, pair terms: the kernel before the force call of a step also does k_prepare's work
+static bool can_prepare(tmd_ctx* ctx) { return priv(ctx).fuse_prepare && ctx->d.own_all && ctx->pair_mask; }
+
+// link: see StepLink.  FOLD where the bonded kernels run on the side stream and the second half-kick can add their sums
+// (k_vv_second_fold, k_cvv_second_fold, k_cstep_boundary); DEFERRED on the cluster path of the whole system without the
+// side stream (k_bonded_vv_second).
+static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double* energies, cudaStream_t st,
+                          StepLink* link = nullptr) {
   DeviceState& d = ctx->d;
   const int N = ctx->natoms, R = ctx->nrep;
   ctx->force_calls++;
@@ -1733,24 +1773,15 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
 
   if (ctx->pair_mask) {
     // Being captured into a CUDA graph?  Then the rebuild becomes the body of a conditional node.
-    cudaGraph_t cap_graph = nullptr;
+    cudaGraph_t cap_graph = capture_graph(ctx, st);
     bool in_body = false;
-    if (priv(ctx).use_graph) {
-      cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-      if (cudaStreamGetCaptureInfo(st, &cs, nullptr, &cap_graph, nullptr, nullptr) != cudaSuccess ||
-          cs != cudaStreamCaptureStatusActive)
-        cap_graph = nullptr;
-    }
     cudaGraphConditionalHandle handle = 0;
-    if (priv(ctx).prepared) {  // k_vv_first_prepare did k_prepare's work (tmd_md_steps)
-      handle = priv(ctx).prepared_cond;
-      priv(ctx).prepared = false;
+    if (link && link->prepared) {
+      handle = link->cond;
     } else {
       DeviceState dp = d;  // k_prepare's copy carries the handle it switches on
-      if (cap_graph) {
-        TMD_CUDA(cudaGraphConditionalHandleCreate(&handle, cap_graph, 0, cudaGraphCondAssignDefault));
-        dp.cond = (unsigned long long)handle;
-      }
+      if (int rc = capture_cond(ctx, st, dp)) return rc;
+      handle = dp.cond;
       launch(k_prepare, atoms_grid(ctx, 256), 256, st, dp, pos);
       TMD_LAUNCHED(ctx, "k_prepare");
     }
@@ -1841,8 +1872,8 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
   if (overlap) {
     CtxPriv& pv = priv(ctx);
     TMD_CUDA(cudaStreamWaitEvent(st, pv.ev_join, 0));
-    if (pv.fold_next) {  // the integrator kernel that follows adds them (enqueue_vv_second)
-      pv.fold_pending = true;
+    if (link && pv.fuse_prepare) {  // the integrator kernel that follows adds them
+      link->tail = StepLink::FOLD;
     } else if (d.cl.on) {
       launch(k_cadd_bonded, owned_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, d, forces, pv.bonded_scratch);
       TMD_LAUNCHED(ctx, "k_cadd_bonded");
@@ -1850,13 +1881,13 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
       launch(k_add_bonded, owned_grid(ctx, BONDED_THREADS), BONDED_THREADS, st, N, d.own_lo, d.own_n, forces, pv.bonded_scratch);
       TMD_LAUNCHED(ctx, "k_add_bonded");
     }
-  } else if (d.cl.on && ctx->pair_mask && priv(ctx).defer_bonded && d.own_all) {
-    // tmd_md_steps: bonded terms, the trip home from slot order and the second half-kick are one kernel
-    priv(ctx).bonded_deferred = true;
+  } else if (link && d.cl.on && ctx->pair_mask && d.own_all) {
+    // bonded terms, the trip home from slot order and the second half-kick are one kernel
     if (!have_bonded) memset(&T, 0, sizeof(T));
-    priv(ctx).deferred_tables = T;
-    priv(ctx).deferred_energies = energies;
-    priv(ctx).deferred_pos = pos;
+    link->tail = StepLink::DEFERRED;
+    link->T = T;
+    link->pos = pos;
+    link->energies = energies;
   } else if (have_bonded) {
     // (cluster path: this kernel also brings the pair forces home from slot order)
     if (int brc = launch_bonded(st, nullptr)) return brc;
@@ -1866,13 +1897,6 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
   }
   return TMD_OK;
 }
-
-// the step boundary of tmd_md_steps (fused.cuh, k_cstep_boundary): what enqueue_vv_second + enqueue_vv_first would do
-struct BoundaryArgs {
-  double gamma;
-  const float* vcoeff;
-  uint64_t seed, step;
-};
 
 // ---- constraints (constrain.cuh) ------------------------------------------------------------
 static inline bool has_constraints(tmd_ctx* ctx) { return priv(ctx).con_ngroups > 0; }
@@ -1895,28 +1919,19 @@ static int enqueue_constrain_pos(tmd_ctx* ctx, T* pos, const T* ref, T* vel, con
   TMD_LAUNCHED(ctx, "k_constrain_pos");
   return TMD_OK;
 }
-// tmd_md_steps (fp32, whole system, TMD_B200_FUSEPREP): the position constraint also prepares the force call that
-// follows on this stream (list check, slot records), as k_vv_first_prepare does without constraints
-static bool con_can_prepare(tmd_ctx* ctx) { return priv(ctx).fuse_prepare && ctx->d.own_all && ctx->pair_mask; }
+// tmd_md_steps (fp32, can_prepare): the position constraint also prepares the force call that follows on this stream
+// (list check, slot records), as k_vv_first_prepare does without constraints
 static int enqueue_constrain_pos_prepare(tmd_ctx* ctx, float* pos, const float* ref, float* vel, const float* masses, double dt,
-                                         cudaStream_t st) {
+                                         cudaStream_t st, StepLink& link) {
   CtxPriv& pv = priv(ctx);
   DeviceState dp = ctx->d;
-  pv.prepared_cond = 0;
-  if (pv.use_graph) {
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    cudaGraph_t cap_graph = nullptr;
-    if (cudaStreamGetCaptureInfo(st, &cs, nullptr, &cap_graph, nullptr, nullptr) == cudaSuccess &&
-        cs == cudaStreamCaptureStatusActive && cap_graph) {
-      TMD_CUDA(cudaGraphConditionalHandleCreate(&pv.prepared_cond, cap_graph, 0, cudaGraphCondAssignDefault));
-      dp.cond = (unsigned long long)pv.prepared_cond;
-    }
-  }
+  if (int rc = capture_cond(ctx, st, dp)) return rc;
   const dim3 g((pv.con_ngroups + pv.con_nfree + CON_THREADS - 1) / CON_THREADS, ctx->nrep);
   launch(k_constrain_pos<float, true>, g, CON_THREADS, st, ctx->natoms, con_tables(ctx), pos, ref, vel, masses, 1.0 / dt,
          pv.con_fail, dp);
   TMD_LAUNCHED(ctx, "k_constrain_pos");
-  pv.prepared = true;
+  link.prepared = true;
+  link.cond = dp.cond;
   return TMD_OK;
 }
 // velocity projection; with ke, the kinetic energy after it
@@ -1935,36 +1950,27 @@ static int enqueue_constrain_vel(tmd_ctx* ctx, const T* pos, T* vel, const T* ma
   return TMD_OK;
 }
 
+// link != nullptr: the force call of a step follows on this stream, and where can_prepare it finds its preparation
+// done.  boundary (the arguments of the tmd_md_steps call): k_cstep_boundary (fused.cuh) instead, which is also the
+// second half-kick of the step before, whose force call left its fold to this kernel.
 static int enqueue_vv_first(tmd_ctx* ctx, float* pos, float* vel, const float* forces, const float* masses,
-                            double dt, cudaStream_t st, bool forces_follow = false, const BoundaryArgs* boundary = nullptr) {
-  CtxPriv& pv = priv(ctx);
-  if (forces_follow && pv.fuse_prepare && ctx->d.own_all && ctx->pair_mask) {
-    // the force call that follows on this stream finds its preparation done
+                            double dt, cudaStream_t st, StepLink* link = nullptr, const StepArgs* boundary = nullptr) {
+  if (link && can_prepare(ctx)) {
     DeviceState dp = ctx->d;
-    pv.prepared_cond = 0;
-    if (pv.use_graph) {
-      cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-      cudaGraph_t cap_graph = nullptr;
-      if (cudaStreamGetCaptureInfo(st, &cs, nullptr, &cap_graph, nullptr, nullptr) == cudaSuccess &&
-          cs == cudaStreamCaptureStatusActive && cap_graph) {
-        TMD_CUDA(cudaGraphConditionalHandleCreate(&pv.prepared_cond, cap_graph, 0, cudaGraphCondAssignDefault));
-        dp.cond = (unsigned long long)pv.prepared_cond;
-      }
-    }
-    if (boundary) {  // the force call before left its fold to us (fold_pending)
-      pv.fold_pending = false;
-      const bool thermo = (boundary->gamma >= 0.0) && boundary->vcoeff != nullptr;
+    if (int rc = capture_cond(ctx, st, dp)) return rc;
+    link->prepared = true;
+    link->cond = dp.cond;
+    if (boundary) {
       const float fdt = (float)dt, hdt = (float)(0.5 * dt), ng = (float)(-boundary->gamma);
-      if (thermo) launch(k_cstep_boundary<true>, atoms_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, dp, pos, vel, masses, fdt, hdt, ng, boundary->vcoeff, boundary->seed, boundary->step, pv.bonded_scratch);
-      else launch(k_cstep_boundary<false>, atoms_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, dp, pos, vel, masses, fdt, hdt, ng, boundary->vcoeff, boundary->seed, boundary->step, pv.bonded_scratch);
+      const bool thermo = (boundary->gamma >= 0.0) && boundary->vcoeff != nullptr;
+      launch(thermo ? k_cstep_boundary<true> : k_cstep_boundary<false>, atoms_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, dp,
+             pos, vel, masses, fdt, hdt, ng, boundary->vcoeff, boundary->seed, boundary->first_step, priv(ctx).bonded_scratch);
       TMD_LAUNCHED(ctx, "k_cstep_boundary");
-      pv.prepared = true;
       return TMD_OK;
     }
     launch(k_vv_first_prepare, atoms_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, dp, pos, vel, forces, masses, (float)dt,
            (float)(0.5 * dt));
     TMD_LAUNCHED(ctx, "k_vv_first_prepare");
-    pv.prepared = true;
     return TMD_OK;
   }
   launch(k_vv_first, owned_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, 
@@ -1973,65 +1979,87 @@ static int enqueue_vv_first(tmd_ctx* ctx, float* pos, float* vel, const float* f
   return TMD_OK;
 }
 
+// link: the second half-kick of a step also finishes what the step's force call left (StepLink::tail)
 static int enqueue_vv_second(tmd_ctx* ctx, float* vel, const float* forces, const float* masses, double dt,
                              double gamma, const float* vcoeff, const float* noise, uint64_t seed,
-                             uint64_t step, double* ke, cudaStream_t st) {
+                             uint64_t step, double* ke, cudaStream_t st, const StepLink* link = nullptr) {
   const bool thermo = (gamma >= 0.0) && vcoeff != nullptr;
   const dim3 g = owned_grid(ctx, INTEG_THREADS);
   const int lo = ctx->d.own_lo, cnt = ctx->d.own_n;
   const unsigned long long* ctr = ctx->d.counters;
   const float fdt = (float)dt, hdt = (float)(0.5 * dt), ng = (float)(-gamma);
   if (ke) TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
-  if (priv(ctx).bonded_deferred) {
-    CtxPriv& pv = priv(ctx);
-    pv.bonded_deferred = false;
-    float* fw = const_cast<float*>(forces);  // (tmd_md_steps owns this buffer: the force call's output)
-    const dim3 gb = atoms_grid(ctx, BONDED_THREADS);
-    const BondedTables& T = pv.deferred_tables;
-    if (thermo) {
-      if (ke) launch(k_bonded_vv_second<true, true>, gb, BONDED_THREADS, st, ctx->d, T, ctx->q, pv.deferred_pos, fw, pv.deferred_energies, vel, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke);
-      else launch(k_bonded_vv_second<true, false>, gb, BONDED_THREADS, st, ctx->d, T, ctx->q, pv.deferred_pos, fw, pv.deferred_energies, vel, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke);
-    } else {
-      if (ke) launch(k_bonded_vv_second<false, true>, gb, BONDED_THREADS, st, ctx->d, T, ctx->q, pv.deferred_pos, fw, pv.deferred_energies, vel, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke);
-      else launch(k_bonded_vv_second<false, false>, gb, BONDED_THREADS, st, ctx->d, T, ctx->q, pv.deferred_pos, fw, pv.deferred_energies, vel, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke);
-    }
+  const StepLink::Tail tail = link ? link->tail : StepLink::NONE;
+  float* fw = const_cast<float*>(forces);  // (FOLD, DEFERRED: tmd_md_steps owns this buffer, the force call's output)
+  if (tail == StepLink::DEFERRED) {
+    with_bools(thermo, ke != nullptr, [&](auto th, auto e) {
+      launch(k_bonded_vv_second<th, e>, atoms_grid(ctx, BONDED_THREADS), BONDED_THREADS, st, ctx->d, link->T, ctx->q, link->pos, fw,
+             link->energies, vel, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke);
+    });
     TMD_LAUNCHED(ctx, "k_bonded_vv_second");
     return TMD_OK;
   }
-  if (priv(ctx).fold_pending) {
-    priv(ctx).fold_pending = false;
-    float* fw = const_cast<float*>(forces);  // (tmd_md_steps owns this buffer: it handed it to enqueue_forces as the output)
-    const double* sc = priv(ctx).bonded_scratch;
-    if (ctx->d.cl.on) {  // cluster path: the pair forces come home from slot order on the way
-      if (thermo) {
-        if (ke) launch(k_cvv_second_fold<true, true>, g, INTEG_THREADS, st, ctx->d, vel, fw, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke, sc);
-        else launch(k_cvv_second_fold<true, false>, g, INTEG_THREADS, st, ctx->d, vel, fw, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke, sc);
-      } else {
-        if (ke) launch(k_cvv_second_fold<false, true>, g, INTEG_THREADS, st, ctx->d, vel, fw, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke, sc);
-        else launch(k_cvv_second_fold<false, false>, g, INTEG_THREADS, st, ctx->d, vel, fw, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke, sc);
-      }
-      TMD_LAUNCHED(ctx, "k_cvv_second_fold");
-      return TMD_OK;
-    }
-    if (thermo) {
-      if (ke) launch(k_vv_second_fold<true, true>, g, INTEG_THREADS, st, ctx->natoms, lo, cnt, ctr, vel, fw, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke, sc);
-      else launch(k_vv_second_fold<true, false>, g, INTEG_THREADS, st, ctx->natoms, lo, cnt, ctr, vel, fw, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke, sc);
-    } else {
-      if (ke) launch(k_vv_second_fold<false, true>, g, INTEG_THREADS, st, ctx->natoms, lo, cnt, ctr, vel, fw, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke, sc);
-      else launch(k_vv_second_fold<false, false>, g, INTEG_THREADS, st, ctx->natoms, lo, cnt, ctr, vel, fw, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke, sc);
-    }
+  const double* sc = priv(ctx).bonded_scratch;
+  if (tail == StepLink::FOLD && ctx->d.cl.on) {  // cluster path: the pair forces come home from slot order on the way
+    with_bools(thermo, ke != nullptr, [&](auto th, auto e) {
+      launch(k_cvv_second_fold<th, e>, g, INTEG_THREADS, st, ctx->d, vel, fw, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke, sc);
+    });
+    TMD_LAUNCHED(ctx, "k_cvv_second_fold");
+    return TMD_OK;
+  }
+  if (tail == StepLink::FOLD) {
+    with_bools(thermo, ke != nullptr, [&](auto th, auto e) {
+      launch(k_vv_second_fold<th, e>, g, INTEG_THREADS, st, ctx->natoms, lo, cnt, ctr, vel, fw, masses, fdt, hdt, ng, vcoeff, noise,
+             seed, step, ke, sc);
+    });
     TMD_LAUNCHED(ctx, "k_vv_second_fold");
     return TMD_OK;
   }
-  if (thermo) {
-    if (ke) launch(k_vv_second<true, true>, g, INTEG_THREADS, st, ctx->natoms, lo, cnt, ctr, vel, forces, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke);
-    else launch(k_vv_second<true, false>, g, INTEG_THREADS, st, ctx->natoms, lo, cnt, ctr, vel, forces, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke);
-  } else {
-    if (ke) launch(k_vv_second<false, true>, g, INTEG_THREADS, st, ctx->natoms, lo, cnt, ctr, vel, forces, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke);
-    else launch(k_vv_second<false, false>, g, INTEG_THREADS, st, ctx->natoms, lo, cnt, ctr, vel, forces, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke);
-  }
+  with_bools(thermo, ke != nullptr, [&](auto th, auto e) {
+    launch(k_vv_second<th, e>, g, INTEG_THREADS, st, ctx->natoms, lo, cnt, ctr, vel, forces, masses, fdt, hdt, ng, vcoeff, noise,
+           seed, step, ke);
+  });
   TMD_LAUNCHED(ctx, "k_vv_second");
   return TMD_OK;
+}
+
+// One step of tmd_md_steps: whether it opens with k_cstep_boundary (which finishes the step before), writes the
+// energies, and closes with its second half-kick; and its slice of the injected noise.
+struct StepShape {
+  bool boundary, energies, closes;
+  const float* noise;
+};
+// the captured steps CtxPriv::exec[0..4]
+static constexpr StepShape STEP_VARIANTS[CtxPriv::NGRAPH] = {
+    {false, false, true, nullptr}, {false, true, true, nullptr}, {false, false, false, nullptr},
+    {true, false, false, nullptr}, {true, true, true, nullptr}};
+// which of them step `it` of a call of niter steps is (fuse: TMD_B200_FUSESTEP applies, niter >= 2)
+static int step_variant(bool fuse, int it, int niter) {
+  const bool last = it == niter - 1;
+  return fuse ? (it == 0 ? 2 : (last ? 4 : 3)) : (last ? 1 : 0);
+}
+
+// Enqueues one MD step, the captured ones and those of the stream path alike: the first half-kick and drift (or
+// k_cstep_boundary), with constraints the position constraint, the force call, then the second half-kick and the
+// velocity constraint.  The kernels hand each other their work through a StepLink local to the step.
+static int enqueue_step(tmd_ctx* ctx, const StepArgs& a, const StepShape& shape, cudaStream_t st) {
+  const bool con = has_constraints(ctx);
+  const float* cref = static_cast<const float*>(priv(ctx).con_ref);
+  StepLink link;
+  int rc;
+  if (con && (rc = con_save_ref(ctx, a.pos, st))) return rc;
+  if ((rc = enqueue_vv_first(ctx, a.pos, a.vel, a.forces, a.masses, a.dt, st, con ? nullptr : &link, shape.boundary ? &a : nullptr)))
+    return rc;
+  if (con && (rc = can_prepare(ctx) ? enqueue_constrain_pos_prepare(ctx, a.pos, cref, a.vel, a.masses, a.dt, st, link)
+                                    : enqueue_constrain_pos(ctx, a.pos, cref, a.vel, a.masses, a.dt, st)))
+    return rc;
+  if ((rc = enqueue_forces(ctx, a.pos, a.forces, shape.energies ? a.energies : nullptr, st, &link))) return rc;
+  if (!shape.closes)  // the next step's k_cstep_boundary finishes this one: it adds the bonded sums
+    return link.tail == StepLink::FOLD ? TMD_OK : fail(TMD_ERR_STATE, "tmd_md_steps: a step left open has no bonded fold for the next one");
+  if ((rc = enqueue_vv_second(ctx, a.vel, a.forces, a.masses, a.dt, a.gamma, a.vcoeff, shape.noise, a.seed, a.first_step,
+                              shape.energies && !con ? a.ke : nullptr, st, &link)))
+    return rc;
+  return con ? enqueue_constrain_vel(ctx, a.pos, a.vel, a.masses, shape.energies ? a.ke : nullptr, st) : TMD_OK;
 }
 
 extern "C" {
@@ -2043,7 +2071,6 @@ int tmd_forces(tmd_ctx* ctx, const float* pos, float* forces, double* energies, 
   cudaStream_t st = (cudaStream_t)stream;
   int rc;
   if (priv(ctx).dirty && (rc = finalize(ctx, st))) return rc;
-  priv(ctx).prepared = false;  // (only tmd_md_steps prepares ahead of the force call)
   return enqueue_forces(ctx, pos, forces, energies, st);
 }
 
@@ -2096,19 +2123,6 @@ int tmd_md_steps(tmd_ctx* ctx, int niter, float* pos, float* vel, float* forces,
   if (priv(ctx).dirty && (rc = finalize(ctx, st))) return rc;
   const size_t per_step = (size_t)ctx->nrep * ctx->natoms * 3;
   CtxPriv& pv = priv(ctx);
-  pv.prepared = false;
-  pv.fold_pending = false;
-  pv.bonded_deferred = false;
-  struct DeferScope {  // only inside tmd_md_steps does a vv_second follow every force call
-    CtxPriv& p;
-    explicit DeferScope(CtxPriv& q) : p(q) { p.defer_bonded = true; }
-    ~DeferScope() { p.defer_bonded = false; }
-  } defer_scope(pv);
-  struct FoldScope {  // only inside tmd_md_steps does a vv_second follow every force call
-    CtxPriv& p;
-    explicit FoldScope(CtxPriv& q, bool on) : p(q) { p.fold_next = on; }
-    ~FoldScope() { p.fold_next = false; }
-  } fold_scope(pv, pv.fuse_prepare);
   // TMD_B200_FUSESTEP: inside one call the second half of a step and the first half of the next are one kernel
   // (cluster path with the bonded kernel on the side stream: the force call leaves its fold to the integrator)
   // With constraints the step is RATTLE: the position constraint sits between the drift and the force call and the
@@ -2116,9 +2130,8 @@ int tmd_md_steps(tmd_ctx* ctx, int niter, float* pos, float* vel, float* forces,
   const bool con = has_constraints(ctx);
   const bool fuse = pv.fuse_step && pv.fuse_prepare && ctx->d.cl.on && ctx->d.own_all && ctx->pair_mask && !noise &&
                     ctx->bonded_nentries > 0 && pv.side != nullptr && niter >= 2 && !con;
-  const float* cref = static_cast<const float*>(pv.con_ref);
   if (con) pv.con_pos = pos;
-  const BoundaryArgs bargs{gamma, vcoeff, seed, first_step};
+  const StepArgs args{pos, vel, forces, masses, vcoeff, dt, gamma, seed, first_step, energies, ke};
   if (pv.use_graph && !noise && !pv.profiling && niter > 0) {
     // One MD step captured once (with and without the energy outputs) and replayed: one graph
     // launch per step, the rebuild kernels inside a conditional node.  Everything that changes
@@ -2127,8 +2140,7 @@ int tmd_md_steps(tmd_ctx* ctx, int niter, float* pos, float* vel, float* forces,
     cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
     cudaStreamIsCapturing(st, &cs);
     if (cs == cudaStreamCaptureStatusNone) {
-      const CtxPriv::StepKey key{pos, vel, forces, masses, vcoeff, dt, gamma, seed, first_step, energies, ke};
-      if (!pv.steps_valid || memcmp(&key, &pv.step_key, sizeof(key)) != 0 || memcmp(&ctx->d, &pv.step_state, sizeof(DeviceState)) != 0) {
+      if (!pv.steps_valid || memcmp(&args, &pv.step_key, sizeof(args)) != 0 || memcmp(&ctx->d, &pv.step_state, sizeof(DeviceState)) != 0) {
         for (int k = 0; k < CtxPriv::NGRAPH; ++k) {
           if (pv.exec[k]) cudaGraphExecDestroy(pv.exec[k]);
           if (pv.graph[k]) cudaGraphDestroy(pv.graph[k]);
@@ -2137,23 +2149,11 @@ int tmd_md_steps(tmd_ctx* ctx, int niter, float* pos, float* vel, float* forces,
         }
         pv.steps_valid = false;
       }
-      // variants: 0 whole step, 1 whole step + energies, 2 first step without its second half-kick,
-      // 3 boundary + force call, 4 boundary + force call with energies + second half-kick with the kinetic energy
       auto capture = [&](int k) -> int {
         if (pv.exec[k]) return TMD_OK;
-        const bool with_e = (k == 1 || k == 4), opens_with_boundary = (k >= 3), closes = (k != 2 && k != 3);
         const int64_t l0 = ctx->launches, f0 = ctx->force_calls;
         TMD_CUDA(cudaStreamBeginCapture(pv.gstream, cudaStreamCaptureModeRelaxed));
-        int rc2 = con ? con_save_ref(ctx, pos, pv.gstream) : TMD_OK;
-        if (!rc2) rc2 = enqueue_vv_first(ctx, pos, vel, forces, masses, dt, pv.gstream, !con, opens_with_boundary ? &bargs : nullptr);
-        if (!rc2 && con)
-          rc2 = con_can_prepare(ctx) ? enqueue_constrain_pos_prepare(ctx, pos, cref, vel, masses, dt, pv.gstream)
-                                     : enqueue_constrain_pos(ctx, pos, cref, vel, masses, dt, pv.gstream);
-        if (!rc2) rc2 = enqueue_forces(ctx, pos, forces, with_e ? energies : nullptr, pv.gstream);
-        if (!rc2 && closes) rc2 = enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, nullptr, seed, first_step,
-                                                    with_e && !con ? ke : nullptr, pv.gstream);
-        if (!rc2 && closes && con) rc2 = enqueue_constrain_vel(ctx, pos, vel, masses, with_e ? ke : nullptr, pv.gstream);
-        pv.fold_pending = false;  // (variants 2 and 3 leave the fold to the graph that follows)
+        const int rc2 = enqueue_step(ctx, args, STEP_VARIANTS[k], pv.gstream);
         cudaError_t ce = cudaStreamEndCapture(pv.gstream, &pv.graph[k]);
         if (rc2) return rc2;
         if (ce != cudaSuccess) return fail(TMD_ERR_CUDA, std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce));
@@ -2173,14 +2173,14 @@ int tmd_md_steps(tmd_ctx* ctx, int niter, float* pos, float* vel, float* forces,
       }
       if (!pv.steps_valid) {
         memset(&pv.step_key, 0, sizeof(pv.step_key));
-        pv.step_key = key;
+        pv.step_key = args;
         pv.step_state = ctx->d;
         pv.steps_valid = true;
       }
       TMD_CUDA(cudaEventRecord(pv.ev_in, st));
       TMD_CUDA(cudaStreamWaitEvent(pv.gstream, pv.ev_in, 0));
       for (int it = 0; it < niter; ++it) {
-        const int k = fuse ? (it == 0 ? 2 : (it == niter - 1 ? 4 : 3)) : (it == niter - 1 ? 1 : 0);
+        const int k = step_variant(fuse, it, niter);
         TMD_CUDA(cudaGraphLaunch(pv.exec[k], pv.gstream));
         ctx->launches += pv.step_launches[k];
       }
@@ -2191,18 +2191,9 @@ int tmd_md_steps(tmd_ctx* ctx, int niter, float* pos, float* vel, float* forces,
     }
   }
   for (int it = 0; it < niter; ++it) {
-    const bool last = (it == niter - 1);
-    if (con && (rc = con_save_ref(ctx, pos, st))) return rc;
-    if ((rc = enqueue_vv_first(ctx, pos, vel, forces, masses, dt, st, !con, fuse && it > 0 ? &bargs : nullptr))) return rc;
-    if (con && (rc = con_can_prepare(ctx) ? enqueue_constrain_pos_prepare(ctx, pos, cref, vel, masses, dt, st)
-                                          : enqueue_constrain_pos(ctx, pos, cref, vel, masses, dt, st)))
-      return rc;
-    if ((rc = enqueue_forces(ctx, pos, forces, last ? energies : nullptr, st))) return rc;
-    if (fuse && !last) continue;  // the next iteration's boundary kernel finishes this step
-    if ((rc = enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise ? noise + it * per_step : nullptr,
-                                seed, first_step, last && !con ? ke : nullptr, st)))
-      return rc;
-    if (con && (rc = enqueue_constrain_vel(ctx, pos, vel, masses, last ? ke : nullptr, st))) return rc;
+    StepShape shape = STEP_VARIANTS[step_variant(fuse, it, niter)];
+    shape.noise = noise ? noise + it * per_step : nullptr;
+    if ((rc = enqueue_step(ctx, args, shape, st))) return rc;
   }
   return TMD_OK;
 }
@@ -2255,13 +2246,9 @@ static void enqueue_vv_second_f64(tmd_ctx* ctx, double* vel, const double* force
   const dim3 g = atoms_grid(ctx, INTEG_THREADS);
   const int n = ctx->natoms;
   const unsigned long long* ctr = ctx->d.counters;
-  if (thermo) {
-    if (ke) launch(k_vv_second_f64<true, true>, g, INTEG_THREADS, st, n, ctr, vel, forces, masses, dt, 0.5 * dt, -gamma, vcoeff, noise, seed, step, ke);
-    else launch(k_vv_second_f64<true, false>, g, INTEG_THREADS, st, n, ctr, vel, forces, masses, dt, 0.5 * dt, -gamma, vcoeff, noise, seed, step, ke);
-  } else {
-    if (ke) launch(k_vv_second_f64<false, true>, g, INTEG_THREADS, st, n, ctr, vel, forces, masses, dt, 0.5 * dt, -gamma, vcoeff, noise, seed, step, ke);
-    else launch(k_vv_second_f64<false, false>, g, INTEG_THREADS, st, n, ctr, vel, forces, masses, dt, 0.5 * dt, -gamma, vcoeff, noise, seed, step, ke);
-  }
+  with_bools(thermo, ke != nullptr, [&](auto th, auto e) {
+    launch(k_vv_second_f64<th, e>, g, INTEG_THREADS, st, n, ctr, vel, forces, masses, dt, 0.5 * dt, -gamma, vcoeff, noise, seed, step, ke);
+  });
 }
 
 int tmd_vv_first_f64(tmd_ctx* ctx, double* pos, double* vel, const double* forces, const double* masses, double dt,
