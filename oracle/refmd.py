@@ -392,13 +392,14 @@ class OracleForces:
 # row-sampled evaluation for systems the all-pairs table cannot hold
 # ----------------------------------------------------------------------------
 def sampled_rows(par, terms, pos, box_diag, atoms, cutoff, rfa=False, solventDielectric=78.5, switch_dist=None,
-                 exclusions=("bonds", "angles", "1-4"), chunk=256):
+                 exclusions=("bonds", "angles", "1-4"), chunk=256, true_gradient=False):
     """Non-bonded force on each atom of ``atoms`` from ALL its partners, and its in-cutoff partner sets.
 
     The reference's pair arithmetic (forces.py:264-319 with 360-372, 381-415, 453-491) restricted to the
     rows of the all-pairs table that contain a sampled atom: 1,000 atoms x 99,999 partners is 1e8 distances,
     where the full table (forces.py:348-357) would need 5e9.  Decisions ``dist <= cutoff`` in fp32 on fp32
-    positions like the reference's fp32 path; values in the dtype of ``pos`` (fp64: the yardstick).
+    positions like the reference's fp32 path; values in the dtype of ``pos`` (fp64: the yardstick).  ``true_gradient``:
+    the switched LJ as the exact gradient of its energy (OracleForces' option of the same name).
     ``pos`` (N,3), ``box_diag`` (3,).  Returns (forces (len(atoms),3), list of sorted partner index arrays)."""
     terms = [t.lower() for t in terms]
     N = pos.shape[0]
@@ -435,7 +436,7 @@ def sampled_rows(par, terms, pos, box_diag, atoms, cutoff, rfa=False, solventDie
         if "lj" in terms:
             a_ = A[types[idx[:, 0]], types[idx[:, 1]]]
             b_ = B[types[idx[:, 0]], types[idx[:, 1]]]
-            dedr += lj_pair(dist, a_, b_, 1, switch_dist, cutoff)[1]
+            dedr += lj_pair(dist, a_, b_, 1, switch_dist, cutoff, true_gradient)[1]
         if "electrostatics" in terms:
             dedr += coulomb_pair(dist, q[idx[:, 0]], q[idx[:, 1]], 1, cutoff, rfa, solventDielectric)[1]
         fvec = unit * dedr.unsqueeze(1)  # forces.py:316-319: f[idx0] -= fvec ; f[idx1] += fvec

@@ -576,7 +576,9 @@ struct ClTab {
 // MINUS the force coefficient (dE/dr)/r of two pairs: pair_coef2 of physics.cuh with the LJ factors 12 A, 6 B
 // taken from the table (two operations fewer).
 // EW: real-space Ewald electrostatics (physics.cuh, ewald_ndedr2) in place of the reaction field.
-template <bool ENERGY, bool EW = false>
+// GRAD: the switched LJ as the exact derivative s dE/dr + E s' of its energy (tmd_set_force_convention 1, the autograd
+// path) in place of the reference's explicit formula.
+template <bool ENERGY, bool EW = false, bool GRAD = false>
 __device__ __forceinline__ F2 cl_coef2(const SwitchConsts& c, F2 s, F2 nqq, const ClTab& t, F2& e_lj, F2& ne_el) {
   const F2 y = f2(rsqrt_seed(s.x), rsqrt_seed(s.y));
   const F2 h = f2_mul(s, y);
@@ -596,7 +598,8 @@ __device__ __forceinline__ F2 cl_coef2(const SwitchConsts& c, F2 s, F2 nqq, cons
   const F2 t2 = f2_mul(tt, tt);
   const F2 sw = f2_fma(f2_mul(t2, tt), f2_fma(tt, f2_fma(tt, f2(-6.0f), f2(15.0f)), f2(-10.0f)), f2(1.0f));
   const F2 ndsw = f2_mul(t2, f2_fma(tt, f2_fma(tt, f2(c.d1), f2(c.d2)), f2(c.d3)));
-  const F2 nfsw = f2_fma(sw, nf, f2_mul(f2_mul(e, ndsw), rinv));  // the reference's s dE/dr + E s'/r (forces.py:410-412)
+  // the reference's s dE/dr + E s'/r (forces.py:410-412), or the exact s dE/dr + E s'
+  const F2 nfsw = GRAD ? f2_fma(sw, nf, f2_mul(e, ndsw)) : f2_fma(sw, nf, f2_mul(f2_mul(e, ndsw), rinv));
   if constexpr (EW) {
     F2 ec;
     const F2 ndedr = f2_add(ewald_ndedr2(c, nqq, r, rinv, nr2, ec), nfsw);
@@ -637,7 +640,7 @@ struct ClExactArgs {
   unsigned terms;
   float s_lo, s_hi, s_max;
 };
-template <bool ENERGY, bool EW>
+template <bool ENERGY, bool EW, bool GRAD>
 __device__ __forceinline__ float2 cl_exact_body(const ClExactArgs& a, int2 mt, const SwitchConsts& sc) {
   const int lane = threadIdx.x & 31;
   const Grid* g = a.g;
@@ -670,7 +673,7 @@ __device__ __forceinline__ float2 cl_exact_body(const ClExactArgs& a, int2 mt, c
             tb.dab = make_float4(12.0f * ab.x, 12.0f * ab.x, 6.0f * ab.y, 6.0f * ab.y);
             const float nqq = (a.terms & T_ELEC) ? -(__int_as_float(pi.w) * __int_as_float(pj.w)) : 0.f;
             F2 elj, neel;
-            const F2 nc = cl_coef2<ENERGY, EW>(sc, f2(s), f2(nqq), tb, elj, neel);
+            const F2 nc = cl_coef2<ENERGY, EW, GRAD>(sc, f2(s), f2(nqq), tb, elj, neel);
             red_add_f32x4(a.f + si, wx * nc.x, wy * nc.x, wz * nc.x);
             red_add_f32x4(a.f + sj, -wx * nc.x, -wy * nc.x, -wz * nc.x);
             if (ENERGY) {
@@ -691,15 +694,20 @@ __device__ __forceinline__ float2 cl_exact_body(const ClExactArgs& a, int2 mt, c
 }
 template <bool ENERGY>
 __device__ __noinline__ float2 cl_exact_pass(ClExactArgs a, int2 mt, SwitchConsts sc) {
-  return cl_exact_body<ENERGY, false>(a, mt, sc);
+  return cl_exact_body<ENERGY, false, false>(a, mt, sc);
 }
 template <bool ENERGY>
 __device__ __noinline__ float2 cl_exact_pass_ew(ClExactArgs a, int2 mt, SwitchConsts sc) {
-  return cl_exact_body<ENERGY, true>(a, mt, sc);
+  return cl_exact_body<ENERGY, true, false>(a, mt, sc);
+}
+// the exact-gradient convention (separate names: the explicit-convention functions above stay as they were)
+template <bool ENERGY, bool EW>
+__device__ __noinline__ float2 cl_exact_pass_grad(ClExactArgs a, int2 mt, SwitchConsts sc) {
+  return cl_exact_body<ENERGY, EW, true>(a, mt, sc);
 }
 
 // dynamic shared memory: per warp two entry buffers of (mcap + ecap) words, then per warp the LJ table (ntypes x CL_H)
-template <bool ENERGY, bool PERIODIC, bool EW>
+template <bool ENERGY, bool PERIODIC, bool EW, bool GRAD>
 __device__ __forceinline__ void cpair_body(const DeviceState& S, const SwitchConsts& sc, double* __restrict__ energies) {
 #if defined(TMD_SIMT_HOST)
   __shared__ __attribute__((aligned(128))) unsigned char cl_dyn[CL_SMEM_MAX];  // (interpreter build: no dynamic window)
@@ -907,7 +915,7 @@ __device__ __forceinline__ void cpair_body(const DeviceState& S, const SwitchCon
         const ClTab tb = tab[tj * CL_H + p];
         const F2 nqq = f2_mul(NQI[p], f2(qj));
         F2 elj, neel;
-        F2 nc = cl_coef2<ENERGY, EW>(sc, s, nqq, tb, elj, neel);
+        F2 nc = cl_coef2<ENERGY, EW, GRAD>(sc, s, nqq, tb, elj, neel);
         nc = f2(in0 ? nc.x : 0.f, in1 ? nc.y : 0.f);  // a select: the other half may hold inf / NaN
         FX[p] = f2_fma(dx, nc, FX[p]);
         FY[p] = f2_fma(dy, nc, FY[p]);
@@ -988,7 +996,8 @@ __device__ __forceinline__ void cpair_body(const DeviceState& S, const SwitchCon
       a.s_lo = s_in;
       a.s_hi = s_hi;
       a.s_max = S.pp.s_max;
-      const float2 ee = EW ? cl_exact_pass_ew<ENERGY>(a, mt_cur, sc) : cl_exact_pass<ENERGY>(a, mt_cur, sc);
+      const float2 ee = GRAD ? cl_exact_pass_grad<ENERGY, EW>(a, mt_cur, sc)
+                        : EW ? cl_exact_pass_ew<ENERGY>(a, mt_cur, sc) : cl_exact_pass<ENERGY>(a, mt_cur, sc);
       ex_lj += ee.x;
       ex_el += ee.y;
     }
@@ -1012,13 +1021,25 @@ __device__ __forceinline__ void cpair_body(const DeviceState& S, const SwitchCon
 template <bool ENERGY, bool PERIODIC>
 __global__ void __launch_bounds__(CL_WARPS * 32, CL_MINBLOCKS)
 k_cpair(DeviceState S, SwitchConsts sc, double* __restrict__ energies) {
-  cpair_body<ENERGY, PERIODIC, false>(S, sc, energies);
+  cpair_body<ENERGY, PERIODIC, false, false>(S, sc, energies);
 }
 // particle-mesh Ewald contexts (periodic only): real-space Ewald electrostatics (sc from make_switch_consts_ewald)
 template <bool ENERGY>
 __global__ void __launch_bounds__(CL_WARPS * 32, CL_MINBLOCKS)
 k_cpair_ew(DeviceState S, SwitchConsts sc, double* __restrict__ energies) {
-  cpair_body<ENERGY, true, true>(S, sc, energies);
+  cpair_body<ENERGY, true, true, false>(S, sc, energies);
+}
+// The same two kernels in the exact-gradient convention (tmd_set_force_convention 1: the autograd path), chosen per
+// launch, so a context keeps its cluster lists whichever convention a call asks for.
+template <bool ENERGY, bool PERIODIC>
+__global__ void __launch_bounds__(CL_WARPS * 32, CL_MINBLOCKS)
+k_cpair_grad(DeviceState S, SwitchConsts sc, double* __restrict__ energies) {
+  cpair_body<ENERGY, PERIODIC, false, true>(S, sc, energies);
+}
+template <bool ENERGY>
+__global__ void __launch_bounds__(CL_WARPS * 32, CL_MINBLOCKS)
+k_cpair_ew_grad(DeviceState S, SwitchConsts sc, double* __restrict__ energies) {
+  cpair_body<ENERGY, true, true, true>(S, sc, energies);
 }
 
 // forces[i] = pair force of the atom's slot  (systems without bonded terms; otherwise k_bonded_sum adds on the way)

@@ -1155,13 +1155,14 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   d.rlist2 = has_cut ? (float)(rl * rl) : INFINITY;
   d.trigger2 = has_cut ? (float)(0.25 * ctx->skin * ctx->skin) : INFINITY;
 
-  // Cluster half-list path (cluster.cuh): a cutoff, pair terms out of {lj, electrostatics}, explicit-force
-  // convention, few atom types, the whole system on this context; in a periodic box additionally every pair a list
-  // can hold must have ONE image within reach (size condition below).  Otherwise: full Verlet rows.
+  // Cluster half-list path (cluster.cuh): a cutoff, pair terms out of {lj, electrostatics}, few atom types, the
+  // whole system on this context; in a periodic box additionally every pair a list can hold must have ONE image within
+  // reach (size condition below).  Otherwise: full Verlet rows.  Either force convention: the launch picks the
+  // kernel, so the path never depends on which convention the first call asked for.
   ClusterState& cl = d.cl;
   const double cl_extent = 8.0;  // a periodic box must leave room for clusters at least this long (A)
   bool use_cluster = env_switch("TMD_B200_CLUSTER", TMD_DEFAULT_CLUSTER) == 1 && !f64 && !ctx->cluster_failed && has_cut &&
-                     ctx->pair_mask != 0 && (ctx->pair_mask & ~(T_LJ | T_ELEC)) == 0 && !ctx->exact_gradient &&
+                     ctx->pair_mask != 0 && (ctx->pair_mask & ~(T_LJ | T_ELEC)) == 0 &&
                      d.ntypes <= CL_MAXT && N < (1 << 24) - 4096 * CL;
   double cl_max_extent = INFINITY;
   if (use_cluster && ctx->periodic) {
@@ -1311,9 +1312,12 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
       pv.cl_smem = cl_size.smem;  // (at most CL_SMEM_MAX: decided above)
 #if !defined(TMD_SIMT_HOST)
       int per_sm = 0;
-      const void* kernels[6] = {(const void*)k_cpair<false, false>, (const void*)k_cpair<false, true>,
-                                (const void*)k_cpair<true, false>, (const void*)k_cpair<true, true>,
-                                (const void*)k_cpair_ew<false>, (const void*)k_cpair_ew<true>};
+      const void* kernels[12] = {(const void*)k_cpair<false, false>, (const void*)k_cpair<false, true>,
+                                 (const void*)k_cpair<true, false>, (const void*)k_cpair<true, true>,
+                                 (const void*)k_cpair_ew<false>, (const void*)k_cpair_ew<true>,
+                                 (const void*)k_cpair_grad<false, false>, (const void*)k_cpair_grad<false, true>,
+                                 (const void*)k_cpair_grad<true, false>, (const void*)k_cpair_grad<true, true>,
+                                 (const void*)k_cpair_ew_grad<false>, (const void*)k_cpair_ew_grad<true>};
       for (const void* k : kernels) TMD_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pv.cl_smem));
       TMD_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cpair<false, true>, CL_WARPS * 32, pv.cl_smem));
       pv.cl_blocks = std::max(1, std::min(ctx->nsm * std::max(per_sm, 1), (cl.nclusters_cap + CL_WARPS - 1) / CL_WARPS));
@@ -1838,12 +1842,25 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
     CtxPriv& pv = priv(ctx);
     const bool sample = pv.profiling && (size_t)(pv.ev_used + 2) <= pv.ev.size();
     if (sample) TMD_CUDA(cudaEventRecord(pv.ev[pv.ev_used], st));
+    // (the cluster kernels: the explicit convention, or the exact-gradient instantiations of the same kernels)
+    const bool grad = ctx->exact_gradient != 0;
     if (d.cl.on && pme) {
       ctx->last_pair_kernel = 10;
       const SwitchConsts sc = make_switch_consts_ewald(d.pp);
       const dim3 cg(pv.cl_blocks, R);
-      if (energies) launch_smem(k_cpair_ew<true>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
+      if (grad && energies) launch_smem(k_cpair_ew_grad<true>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
+      else if (grad) launch_smem(k_cpair_ew_grad<false>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
+      else if (energies) launch_smem(k_cpair_ew<true>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
       else launch_smem(k_cpair_ew<false>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
+    } else if (d.cl.on && grad) {
+      ctx->last_pair_kernel = 4;
+      const SwitchConsts sc = make_switch_consts(d.pp);
+      const dim3 cg(pv.cl_blocks, R);
+      const bool e = energies != nullptr;
+      if (e && ctx->periodic) launch_smem(k_cpair_grad<true, true>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
+      else if (e) launch_smem(k_cpair_grad<true, false>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
+      else if (ctx->periodic) launch_smem(k_cpair_grad<false, true>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
+      else launch_smem(k_cpair_grad<false, false>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
     } else if (d.cl.on) {
       ctx->last_pair_kernel = 4;
       const SwitchConsts sc = make_switch_consts(d.pp);

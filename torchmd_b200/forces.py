@@ -358,7 +358,10 @@ class Forces:
         reference) runs the same kernels with the switched-LJ term in its exact-gradient form:
         every other term's explicit force already is the derivative of its energy, the
         reference's explicit switched LJ is not (forces.py:410-412), and autograd returns the
-        true one.  With ``toNumpy=False`` and positions that require grad the returned energies
+        true one.  The convention is chosen per call: one ``Forces`` may alternate between the two,
+        every pair kernel (the cluster lists included) evaluates the one the call asks for, and
+        the pair path it takes does not depend on the first call's convention.
+        With ``toNumpy=False`` and positions that require grad the returned energies
         carry a grad_fn whose backward is -F of that exact-gradient pass, so
         ``Epot.sum().backward()`` and ``torch.vmap`` over a batch of systems work as with the
         reference (the batch is folded into the replica dimension).  Gradients w.r.t.
