@@ -1,7 +1,7 @@
 """The in-kernel Langevin noise restated in numpy: Philox4x32-10 and the two Box-Muller transforms of the kernels.
 
 Written from the definition of Philox4x32-10 (Salmon, Moraes, Dror, Shaw, "Parallel random numbers: as easy as 1, 2,
-3", SC'11) and from the device code (``torchmd_b200/csrc/integrate.cuh`` ``normal3``, ``double.cuh`` ``normal3_f64``),
+3", SC'11) and from the device code (``torchmd_b200/csrc/integrate.cuh`` ``normal3`` on float and on double),
 with vectorised uint64 arithmetic: the draw of every (seed, step, slot) can be computed on the host, exactly, and the
 kernels compared with it draw for draw.
 
@@ -27,7 +27,7 @@ import numpy as np
 M0, M1 = np.uint64(0xD2511F53), np.uint64(0xCD9E8D57)  # round multipliers
 W0, W1 = np.uint64(0x9E3779B9), np.uint64(0xBB67AE85)  # Weyl increments of the key
 MASK32 = np.uint64(0xFFFFFFFF)
-TOP_BIT = np.uint64(0x80000000)  # counter word 1 of the second block of normal3_f64
+TOP_BIT = np.uint64(0x80000000)  # counter word 1 of the second block of the fp64 normal3
 
 F32_BOUND = 2e-6
 F64_BOUND = 1e-14
@@ -102,7 +102,7 @@ def u53(hi, lo):
 
 
 def normal3_f64(seed, step, slot):
-    """The three fp64 N(0,1) draws of ``normal3_f64`` (double.cuh): two Philox blocks, the second with the top bit of
+    """The three fp64 N(0,1) draws of ``normal3`` on double (integrate.cuh): two Philox blocks, the second with the top bit of
     counter word 1 set, four 53-bit uniforms, Box-Muller in fp64.  Array (..., 3) float64."""
     (c0, c1, c2, c3), key = _words(seed, step, slot)
     return box_muller_f64(philox4x32_10((c0, c1, c2, c3), key), philox4x32_10((c0, c1 | TOP_BIT, c2, c3), key))

@@ -1,7 +1,7 @@
 """Cost of the CMAP correction maps: thrombin (tests/golden/thrombin_nobox_rf, the fixture's own settings, Langevin at
 300 K, 1 fs) with 1 and 16 replicas, fp32 and fp64, without and with backbone-like CMAP terms (138, picked by the
 rule in tests/test_gpu_cmap.py, two 24x24 maps).  For each: steps/s of Integrator.step, the
-k_bonded_terms (fp64: k_bonded_terms_f64) time per call from torch.profiler in a run of its own, and the kernel launches
+k_bonded_terms time per call (k_bonded_terms<float> or <double>) from torch.profiler in a run of its own, and the kernel launches
 per step.  Prints the GPU's name and power limit read in the same run, and one JSON line.
 
     python scripts/bench_cmap.py [--steps 2000] [--warmup 200]

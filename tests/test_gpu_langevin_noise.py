@@ -3,8 +3,8 @@
 Every Langevin run without injected noise draws its N(0,1) numbers inside the kernels: Philox4x32-10 keyed on (seed,
 step, slot), then Box-Muller.  The noise of step s of atom i of replica r is ``normal3(seed, first_step + position + s,
 r * N + i)`` on every path, where ``position`` is the context's Philox position before the call (``langevin_noise``).
-Six kernels draw it -- k_vv_second, k_vv_second_fold, k_cvv_second_fold, k_cstep_boundary, k_bonded_vv_second and
-k_vv_second_f64 -- and each one is checked here on the path that runs it.
+Six kernels draw it -- k_vv_second<float>, k_vv_second_fold, k_cvv_second_fold, k_cstep_boundary, k_bonded_vv_second
+and k_vv_second<double> -- and each one is checked here on the path that runs it.
 
 a. Draw for draw.  Masses of 1e20 amu (the force term of a kick is ~1e-23 A/tu), gamma = 0 with T > 0 (the thermostat
    kicks, its friction term is exactly 0), zero start velocities, a per-atom ``vcoeff`` of distinct values and a time
@@ -171,7 +171,7 @@ PATHS = {
     # step(1) repeated and a split call on the default path
     "single_steps": ({}, (1,) * 7, None, False, F32, CLUSTER, 5.0),
     "split_3_4": ({}, (3, 4), None, False, F32, CLUSTER, 17 / 4),
-    # fp64: tmd_md_steps_f64 and the stepwise fp64 path (k_vv_second_f64)
+    # fp64: tmd_md_steps_f64 and the stepwise fp64 path (k_vv_second<double>)
     "fp64": ({}, (7,), None, False, F64, None, 12.0),
     "fp64_split": ({}, (3, 4), None, False, F64, None, 12.0),
     "fp64_stepwise": ({}, (7,), None, True, F64, None, 10.0),

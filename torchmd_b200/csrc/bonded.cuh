@@ -12,6 +12,8 @@
 // slot 0 is owned.  Runs beside the pair kernel on a second stream, or after it (its plain store of the non-bonded
 // force doubles as the zeroing of Forces.compute, forces.py:113-114).
 #pragma once
+#include <type_traits>
+
 #include "context.cuh"
 #include "pair.cuh"
 
@@ -31,12 +33,14 @@ __device__ __forceinline__ void bonded_unpack(unsigned ent, int& kind, int& slot
   kind = (int)(ent >> 29), slot = (int)((ent >> 26) & 7u), t = (int)(ent & 0x3ffffffu);
 }
 
-struct BondedTables {
+// P: type of the positions and parameter rows, float ("precision: single") or double ("precision: double")
+template <typename P>
+struct BondedTablesT {
   const int* atom_ptr;   // (natoms+1) CSR over atoms
   const int* entries;    // bonded_entry(kind, slot, term)
-  BondedSet bonds, angles, torsions[2], pairs14;
+  BondedSetT<P> bonds, angles, torsions[2], pairs14;
   CmapSet cmap;
-  BondedSet ub;  // Urey-Bradley: idx (n,2) = the ends of an angle, prm (n,2) = k_ub, s0
+  BondedSetT<P> ub;  // Urey-Bradley: idx (n,2) = the ends of an angle, prm (n,2) = k_ub, s0
 };
 
 struct BoxView {
@@ -53,6 +57,68 @@ __device__ __forceinline__ BoxView box_of(const DeviceState& S, int r) {
 }
 __device__ __forceinline__ Vec3 load3(const float* p, size_t atom) {
   return {p[atom * 3 + 0], p[atom * 3 + 1], p[atom * 3 + 2]};
+}
+__device__ __forceinline__ Vec3d load3d(const double* p, size_t atom) {
+  return {p[atom * 3 + 0], p[atom * 3 + 1], p[atom * 3 + 2]};
+}
+// Minimum-image difference with the reference's fp64 rounding (decisions and values alike).
+__device__ __forceinline__ Vec3d delta64(Vec3d a, Vec3d b, int periodic, const double* L) {
+  Vec3d d = {sub_rn(a.x, b.x), sub_rn(a.y, b.y), sub_rn(a.z, b.z)};
+  if (periodic) {
+    d.x = min_image64(d.x, L[0]);
+    d.y = min_image64(d.y, L[1]);
+    d.z = min_image64(d.z, L[2]);
+  }
+  return d;
+}
+
+// What the bonded kernels of the two precisions do differently, on one replica; each term body is written once on top
+// of it.  Arg: the kernels' argument the frame is made from (bonded_frame).  The two rinv6 round differently; each
+// precision keeps the product its kernels have always formed.
+template <typename P>
+struct BondedFrame;
+// fp32 positions: values from the fp64 difference of the fp32 coordinates, a bond's cutoff decision on the reference's
+// fp32 difference.
+template <>
+struct BondedFrame<float> {
+  using Arg = const float* __restrict__;  // charges scaled by sqrt(coulomb constant)
+  using V = Vec3;
+  const float* q;
+  BoxView bx;
+  __device__ __forceinline__ Vec3 load(const float* p, size_t atom) const { return load3(p, atom); }
+  __device__ __forceinline__ Vec3d delta(Vec3 a, Vec3 b) const { return delta_f64(a, b, bx.periodic, bx.L); }
+  __device__ __forceinline__ static double dist(const Vec3d& d) { return norm(d); }
+  __device__ __forceinline__ static bool cutoff_on(const DeviceState& S) { return S.pp.has_cutoff; }
+  __device__ __forceinline__ bool within_cutoff(const DeviceState& S, Vec3 a, Vec3 b) const {
+    const Vec3 dref = delta_ref(a, b, bx.periodic, bx.L, bx.invL);
+    return sqrt_rn(norm2_ref(dref.x, dref.y, dref.z)) <= S.pp.cutoff;
+  }
+  __device__ __forceinline__ static double rinv6(double rinv) { return rinv * rinv * rinv * rinv * rinv * rinv; }
+};
+// fp64 positions: the reference's fp64 rounding for the decision and the values.
+template <>
+struct BondedFrame<double> {
+  using Arg = DeviceState64;
+  using V = Vec3d;
+  const double* q;  // charges scaled by sqrt(coulomb constant)
+  const double* L;  // this replica's box
+  int periodic, has_cutoff;
+  double cutoff;
+  __device__ __forceinline__ Vec3d load(const double* p, size_t atom) const { return load3d(p, atom); }
+  __device__ __forceinline__ Vec3d delta(Vec3d a, Vec3d b) const { return delta64(a, b, periodic, L); }
+  __device__ __forceinline__ static double dist(const Vec3d& d) { return sqrt_rn(norm2_ref(d.x, d.y, d.z)); }
+  __device__ __forceinline__ bool cutoff_on(const DeviceState&) const { return has_cutoff; }
+  __device__ __forceinline__ bool within_cutoff(const DeviceState&, Vec3d a, Vec3d b) const { return dist(delta(a, b)) <= cutoff; }
+  __device__ __forceinline__ static double rinv6(double rinv) {
+    const double r2 = rinv * rinv;
+    return r2 * r2 * r2;
+  }
+};
+__device__ __forceinline__ BondedFrame<float> bonded_frame(const DeviceState& S, const float* q, int r) {
+  return {q, box_of(S, r)};
+}
+__device__ __forceinline__ BondedFrame<double> bonded_frame(const DeviceState& S, const DeviceState64& D, int r) {
+  return {D.q, D.L + 3 * r, S.grid[r].periodic, D.pp.has_cutoff, D.pp.cutoff};
 }
 
 struct BondedEnergies {
@@ -112,21 +178,20 @@ __device__ __forceinline__ double cmap_term(const CmapSet& C, int t, const Vec3d
   return e;
 }
 
-__device__ __forceinline__ bool bonded_term(const DeviceState& S, const BondedTables& T, const float* __restrict__ q_scaled,
-                                            const float* __restrict__ pos, size_t base, const BoxView& bx, int kind, int t, TermForces& o) {
+template <typename P>
+__device__ __forceinline__ bool bonded_term(const DeviceState& S, const BondedTablesT<P>& T, const BondedFrame<P>& X,
+                                            const P* __restrict__ pos, size_t base, int kind, int t, TermForces& o) {
+  using V = typename BondedFrame<P>::V;
   if (kind == BK_BOND || kind == BK_UREY_BRADLEY) {
     // E = k (r-r0)^2.  Bonds longer than the cutoff are skipped like the reference (forces.py:128-136); Urey-Bradley
     // terms (the ends of an angle, k_ub and s0) have no reference counterpart and are never cutoff-filtered.
-    const BondedSet& B = kind == BK_BOND ? T.bonds : T.ub;
+    const BondedSetT<P>& B = kind == BK_BOND ? T.bonds : T.ub;
     const int i = B.idx[2 * t], j = B.idx[2 * t + 1];
     o.n = 2, o.atom[0] = i, o.atom[1] = j;
-    const Vec3 pi = load3(pos, base + i), pj = load3(pos, base + j);
-    if (kind == BK_BOND && S.pp.has_cutoff) {
-      const Vec3 dref = delta_ref(pi, pj, bx.periodic, bx.L, bx.invL);
-      if (!(sqrt_rn(norm2_ref(dref.x, dref.y, dref.z)) <= S.pp.cutoff)) return false;  // reference decision
-    }
-    const Vec3d d = delta_f64(pi, pj, bx.periodic, bx.L);
-    const double dist = norm(d);
+    const V pi = X.load(pos, base + i), pj = X.load(pos, base + j);
+    if (kind == BK_BOND && X.cutoff_on(S) && !X.within_cutoff(S, pi, pj)) return false;  // reference decision
+    const Vec3d d = X.delta(pi, pj);
+    const double dist = X.dist(d);
     double dedr;
     bond_term<double>(dist, B.prm[2 * t], B.prm[2 * t + 1], o.e, dedr);
     const Vec3d fv = (dedr / dist) * d;  // force on j; i gets the opposite
@@ -137,22 +202,22 @@ __device__ __forceinline__ bool bonded_term(const DeviceState& S, const BondedTa
   if (kind == BK_ANGLE) {
     const int a0 = T.angles.idx[3 * t], a1 = T.angles.idx[3 * t + 1], a2 = T.angles.idx[3 * t + 2];
     o.n = 3, o.atom[0] = a0, o.atom[1] = a1, o.atom[2] = a2;
-    const Vec3 p1 = load3(pos, base + a1);
-    const Vec3d r21 = delta_f64(load3(pos, base + a0), p1, bx.periodic, bx.L);
-    const Vec3d r23 = delta_f64(load3(pos, base + a2), p1, bx.periodic, bx.L);
+    const V p1 = X.load(pos, base + a1);
+    const Vec3d r21 = X.delta(X.load(pos, base + a0), p1);
+    const Vec3d r23 = X.delta(X.load(pos, base + a2), p1);
     o.e = angle_term<double>(r21, r23, T.angles.prm[2 * t], T.angles.prm[2 * t + 1], o.f[0], o.f[1], o.f[2]);
     return true;
   }
   if (kind == BK_DIHEDRAL || kind == BK_IMPROPER) {
-    const BondedSet& B = T.torsions[kind == BK_IMPROPER];
+    const BondedSetT<P>& B = T.torsions[kind == BK_IMPROPER];
     o.n = 4;
 #pragma unroll
     for (int k = 0; k < 4; ++k) o.atom[k] = B.idx[4 * t + k];
-    const Vec3 p0 = load3(pos, base + o.atom[0]), p1 = load3(pos, base + o.atom[1]);
-    const Vec3 p2 = load3(pos, base + o.atom[2]), p3 = load3(pos, base + o.atom[3]);
-    const Vec3d r12 = delta_f64(p0, p1, bx.periodic, bx.L);
-    const Vec3d r23 = delta_f64(p1, p2, bx.periodic, bx.L);
-    const Vec3d r34 = delta_f64(p2, p3, bx.periodic, bx.L);
+    const V p0 = X.load(pos, base + o.atom[0]), p1 = X.load(pos, base + o.atom[1]);
+    const V p2 = X.load(pos, base + o.atom[2]), p3 = X.load(pos, base + o.atom[3]);
+    const Vec3d r12 = X.delta(p0, p1);
+    const Vec3d r23 = X.delta(p1, p2);
+    const Vec3d r34 = X.delta(p2, p3);
     const TorsionGeom<double> g = torsion_geom(r12, r23, r34);
     double e = 0., coef = 0.;
     for (int m = B.term_ptr[t]; m < B.term_ptr[t + 1]; ++m)
@@ -165,28 +230,27 @@ __device__ __forceinline__ bool bonded_term(const DeviceState& S, const BondedTa
     o.n = 5;
 #pragma unroll
     for (int k = 0; k < 5; ++k) o.atom[k] = T.cmap.idx[5 * t + k];
-    const Vec3 p0 = load3(pos, base + o.atom[0]), p1 = load3(pos, base + o.atom[1]), p2 = load3(pos, base + o.atom[2]);
-    const Vec3 p3 = load3(pos, base + o.atom[3]), p4 = load3(pos, base + o.atom[4]);
-    o.e = cmap_term(T.cmap, t, delta_f64(p0, p1, bx.periodic, bx.L), delta_f64(p1, p2, bx.periodic, bx.L),
-                    delta_f64(p2, p3, bx.periodic, bx.L), delta_f64(p3, p4, bx.periodic, bx.L), o.f);
+    const V p0 = X.load(pos, base + o.atom[0]), p1 = X.load(pos, base + o.atom[1]), p2 = X.load(pos, base + o.atom[2]);
+    const V p3 = X.load(pos, base + o.atom[3]), p4 = X.load(pos, base + o.atom[4]);
+    o.e = cmap_term(T.cmap, t, X.delta(p0, p1), X.delta(p1, p2), X.delta(p2, p3), X.delta(p3, p4), o.f);
     return true;
   }
   // BK_PAIR14 (forces.py:185-236): LJ/scnb with no cutoff or switch, Coulomb/scee, never RF
   const int i = T.pairs14.idx[2 * t], j = T.pairs14.idx[2 * t + 1];
   o.n = 2, o.atom[0] = i, o.atom[1] = j;
-  const Vec3d d = delta_f64(load3(pos, base + i), load3(pos, base + j), bx.periodic, bx.L);
-  const double dist = norm(d);
+  const Vec3d d = X.delta(X.load(pos, base + i), X.load(pos, base + j));
+  const double dist = X.dist(d);
   const double rinv = 1.0 / dist;
-  const float* prm = T.pairs14.prm + 4 * t;  // A, B, scnb, scee
+  const P* prm = T.pairs14.prm + 4 * t;  // A, B, scnb, scee
   double dedr = 0.;
   if (S.pp.terms & T_LJ) {
-    const double r6 = rinv * rinv * rinv * rinv * rinv * rinv;
+    const double r6 = X.rinv6(rinv);
     const double a12 = prm[0] * r6 * r6, b6 = prm[1] * r6;
     o.e = (a12 - b6) / prm[2];
     dedr += (6.0 * b6 - 12.0 * a12) * rinv / prm[2];
   }
   if (S.pp.terms & T_ELEC) {
-    const double e = (double)q_scaled[i] * (double)q_scaled[j] * rinv / prm[3];
+    const double e = (double)X.q[i] * (double)X.q[j] * rinv / prm[3];
     o.e2 = e;
     dedr -= e * rinv;
   }
@@ -206,16 +270,16 @@ __device__ __forceinline__ void book_energy(BondedEnergies& E, int kind, const T
 
 // Sum of the bonded forces on atom a of replica r (fp64), every term of the atom re-evaluated in this thread; energies
 // booked by the atom in slot 0 of each term.  (k_bonded_vv_second: systems whose bonded kernel is not forked.)
-__device__ __forceinline__ Vec3d bonded_force_on_atom(const DeviceState& S, const BondedTables& T, const float* __restrict__ q_scaled,
+__device__ __forceinline__ Vec3d bonded_force_on_atom(const DeviceState& S, const BondedTablesT<float>& T, const float* __restrict__ q_scaled,
                                                       const float* __restrict__ pos, int r, int a, BondedEnergies& E) {
   const size_t base = (size_t)r * S.natoms;
-  const BoxView bx = box_of(S, r);
+  const BondedFrame<float> X = bonded_frame(S, q_scaled, r);
   Vec3d f = {0., 0., 0.};
   for (int p = T.atom_ptr[a]; p < T.atom_ptr[a + 1]; ++p) {
     int kind, slot, t;
     bonded_unpack((unsigned)T.entries[p], kind, slot, t);
     TermForces o;
-    if (!bonded_term(S, T, q_scaled, pos, base, bx, kind, t, o)) continue;
+    if (!bonded_term(S, T, X, pos, base, kind, t, o)) continue;
     f = f + (slot == 0 ? o.f[0] : (slot == 1 ? o.f[1] : (slot == 2 ? o.f[2] : (slot == 3 ? o.f[3] : o.f[4]))));
     if (slot == 0) book_energy(E, kind, o);
   }
@@ -233,7 +297,8 @@ __host__ __device__ __forceinline__ int term_arity(int kind) {
 }
 
 // block-level reduction of the bonded energies into the per-replica slots
-__device__ __forceinline__ void bonded_energy_reduce(const DeviceState& S, const BondedTables& T, int r, const BondedEnergies& E,
+template <typename P>
+__device__ __forceinline__ void bonded_energy_reduce(const DeviceState& S, const BondedTablesT<P>& T, int r, const BondedEnergies& E,
                                                      double* __restrict__ energies, double* red) {
   double* Eo = energies + (size_t)r * TMD_NUM_ENERGIES;
   if (T.bonds.n) block_accumulate<BONDED_THREADS / 32>(E.bond, Eo + TMD_E_BONDS, red);
@@ -246,9 +311,10 @@ __device__ __forceinline__ void bonded_energy_reduce(const DeviceState& S, const
   }
 }
 
-// Pass 1: one thread per term.  Terms none of whose atoms this rank owns are skipped (decomposed runs).
+// Pass 1: one thread per term.  Terms none of whose atoms this rank owns are skipped (decomposed runs, fp32 only).
+template <typename P>
 __global__ void __launch_bounds__(BONDED_THREADS)
-k_bonded_terms(DeviceState S, BondedTables T, TermLayout lay, const float* __restrict__ q_scaled, const float* __restrict__ pos,
+k_bonded_terms(DeviceState S, BondedTablesT<P> T, TermLayout lay, typename BondedFrame<P>::Arg arg, const P* __restrict__ pos,
                double* __restrict__ energies, double* __restrict__ term_f) {
   const int r = blockIdx.y;
   const int g = blockIdx.x * blockDim.x + threadIdx.x;
@@ -261,7 +327,7 @@ k_bonded_terms(DeviceState S, BondedTables T, TermLayout lay, const float* __res
     const int t = g - lay.first[kind];
     const size_t base = (size_t)r * S.natoms;
     TermForces o;
-    const bool acts = bonded_term(S, T, q_scaled, pos, base, box_of(S, r), kind, t, o);
+    const bool acts = bonded_term(S, T, bonded_frame(S, arg, r), pos, base, kind, t, o);
     bool mine = S.own_all, books = S.own_all;
     if (!S.own_all) {
 #pragma unroll
@@ -287,8 +353,9 @@ k_bonded_terms(DeviceState S, BondedTables T, TermLayout lay, const float* __res
 }
 
 // Pass 2: one thread per owned atom adds up its term instances in the order of its list.
+template <typename P>
 __global__ void __launch_bounds__(BONDED_THREADS)
-k_bonded_sum(DeviceState S, BondedTables T, TermLayout lay, const double* __restrict__ term_f, float* __restrict__ forces,
+k_bonded_sum(DeviceState S, BondedTablesT<P> T, TermLayout lay, const double* __restrict__ term_f, P* __restrict__ forces,
              double* __restrict__ scratch) {
   const int r = blockIdx.y;
   const int a = S.own_lo + blockIdx.x * blockDim.x + threadIdx.x;  // owned atoms only
@@ -305,25 +372,31 @@ k_bonded_sum(DeviceState S, BondedTables T, TermLayout lay, const double* __rest
     f.y += v[1];
     f.z += v[2];
   }
-  if (scratch) {
-    // beside the pair kernel on another stream: the fp64 sums go to a scratch buffer, k_add_bonded (or the
-    // integrator kernel) folds them into the forces afterwards (same single rounding)
-    double* o = scratch + (base + a) * 3;
-    o[0] = f.x;
-    o[1] = f.y;
-    o[2] = f.z;
-  } else if (S.cl.on) {
-    // cluster path: the pair forces sit in slot order; this kernel brings them home and adds its own sums
-    const float4 pf = S.cl.f[(size_t)r * (S.cl.slots + 1) + S.cl.inv[base + a]];
-    float* out = forces + (base + a) * 3;
-    out[0] = (float)((double)pf.x + f.x);
-    out[1] = (float)((double)pf.y + f.y);
-    out[2] = (float)((double)pf.z + f.z);
-  } else if (p1 > T.atom_ptr[a]) {
-    float* out = forces + (base + a) * 3;
-    out[0] = (float)((double)out[0] + f.x);
-    out[1] = (float)((double)out[1] + f.y);
-    out[2] = (float)((double)out[2] + f.z);
+  if constexpr (std::is_same<P, float>::value) {  // an fp64 context has neither the side stream nor the cluster path
+    if (scratch) {
+      // beside the pair kernel on another stream: the fp64 sums go to a scratch buffer, k_add_bonded (or the
+      // integrator kernel) folds them into the forces afterwards (same single rounding)
+      double* o = scratch + (base + a) * 3;
+      o[0] = f.x;
+      o[1] = f.y;
+      o[2] = f.z;
+      return;
+    }
+    if (S.cl.on) {
+      // cluster path: the pair forces sit in slot order; this kernel brings them home and adds its own sums
+      const float4 pf = S.cl.f[(size_t)r * (S.cl.slots + 1) + S.cl.inv[base + a]];
+      float* out = forces + (base + a) * 3;
+      out[0] = (float)((double)pf.x + f.x);
+      out[1] = (float)((double)pf.y + f.y);
+      out[2] = (float)((double)pf.z + f.z);
+      return;
+    }
+  }
+  if (p1 > T.atom_ptr[a]) {
+    P* out = forces + (base + a) * 3;
+    out[0] = (P)((double)out[0] + f.x);
+    out[1] = (P)((double)out[1] + f.y);
+    out[2] = (P)((double)out[2] + f.z);
   }
 }
 

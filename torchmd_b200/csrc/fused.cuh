@@ -13,7 +13,7 @@ namespace tmd {
 
 template <bool THERMOSTAT, bool KINETIC>
 __global__ void __launch_bounds__(BONDED_THREADS)
-k_bonded_vv_second(DeviceState S, BondedTables T, const float* __restrict__ q_scaled, const float* __restrict__ pos,
+k_bonded_vv_second(DeviceState S, BondedTablesT<float> T, const float* __restrict__ q_scaled, const float* __restrict__ pos,
                    float* __restrict__ forces, double* __restrict__ energies, float* __restrict__ vel,
                    const float* __restrict__ masses, float dt, float hdt, float neg_gamma, const float* __restrict__ vcoeff,
                    const float* __restrict__ noise, uint64_t seed, uint64_t step_offset, double* __restrict__ ke) {
@@ -34,19 +34,14 @@ k_bonded_vv_second(DeviceState S, BondedTables T, const float* __restrict__ q_sc
     float vc = 0.f;
     if (THERMOSTAT) {
       vc = vcoeff[i];
-      if (noise) {
-        xi[0] = noise[a]; xi[1] = noise[a + 1]; xi[2] = noise[a + 2];
-      } else {
-        normal3(seed, step, slot, xi);
-      }
+      langevin_noise(noise, seed, step, slot, xi);
     }
     float v2 = 0.f;
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
       forces[a + d] = f[d];
       float v = vel[a + d];
-      if (THERMOSTAT) v = add_rn(v, add_rn(mul_rn(mul_rn(neg_gamma, v), dt), mul_rn(xi[d], vc)));
-      v = add_rn(v, mul_rn(hdt, div_rn(f[d], m)));
+      langevin_kick<THERMOSTAT>(v, f[d], m, xi[d], vc, neg_gamma, dt, hdt);
       vel[a + d] = v;
       v2 += v * v;
     }
@@ -92,19 +87,14 @@ k_cvv_second_fold(DeviceState S, float* __restrict__ vel, float* __restrict__ fo
     float vc = 0.f;
     if (THERMOSTAT) {
       vc = vcoeff[i];
-      if (noise) {
-        xi[0] = noise[a]; xi[1] = noise[a + 1]; xi[2] = noise[a + 2];
-      } else {
-        normal3(seed, step, slot, xi);
-      }
+      langevin_noise(noise, seed, step, slot, xi);
     }
     float v2 = 0.f;
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
       forces[a + d] = f[d];
       float v = vel[a + d];
-      if (THERMOSTAT) v = add_rn(v, add_rn(mul_rn(mul_rn(neg_gamma, v), dt), mul_rn(xi[d], vc)));
-      v = add_rn(v, mul_rn(hdt, div_rn(f[d], m)));
+      langevin_kick<THERMOSTAT>(v, f[d], m, xi[d], vc, neg_gamma, dt, hdt);
       vel[a + d] = v;
       v2 += v * v;
     }
@@ -151,13 +141,10 @@ k_cstep_boundary(DeviceState S, float* __restrict__ pos, float* __restrict__ vel
 #pragma unroll
   for (int d = 0; d < 3; ++d) {
     float v = vel[a + d];
-    if (THERMOSTAT) v = add_rn(v, add_rn(mul_rn(mul_rn(neg_gamma, v), dt), mul_rn(xi[d], vc)));
-    const float acc = div_rn(f[d], m);
-    v = add_rn(v, mul_rn(hdt, acc));  // end of step n
-    const float drift = add_rn(mul_rn(v, dt), mul_rn(mul_rn(mul_rn(0.5f, acc), dt), dt));
-    x[d] = add_rn(pos[a + d], drift);
+    const float acc = langevin_kick<THERMOSTAT>(v, f[d], m, xi[d], vc, neg_gamma, dt, hdt);  // end of step n, one a for both
+    x[d] = kick_drift(pos + a + d, v, acc, dt, hdt);
     pos[a + d] = x[d];
-    vel[a + d] = add_rn(v, mul_rn(hdt, acc));
+    vel[a + d] = v;
   }
   prepare_atom(S, r, i, parity, x[0], x[1], x[2]);
 }

@@ -15,24 +15,45 @@ namespace tmd {
 
 constexpr int INTEG_THREADS = 256;
 
-// pos += vel*dt + ((0.5*a)*dt)*dt ;  vel += (0.5*dt)*a ;  a = F/m     (integrator.py:61-64)
+// The per-atom arithmetic of the step, one coordinate at a time, in the reference's operation order with single
+// rounded ops; T = float or double.  Every integrator kernel (here and in fused.cuh) is built from these.
+//
+// First half (integrator.py:61-64), a = F/m: returns *x + (vel*dt + ((0.5*a)*dt)*dt), then vel += (0.5*dt)*a.  (x is
+// read only where the drift is added, after the force and the velocity: the kernels keep their load order.)
+template <typename T>
+__device__ __forceinline__ T kick_drift(const T* x, T& v, T acc, T dt, T hdt) {
+  const T drift = add_rn(mul_rn(v, dt), mul_rn(mul_rn(mul_rn(T(0.5), acc), dt), dt));
+  const T xn = add_rn(*x, drift);
+  v = add_rn(v, mul_rn(hdt, acc));
+  return xn;
+}
+// Second half (integrator.py:72-74 then 67-69): [vel += ((-gamma*vel)*dt + xi*vcoeff)], then vel += (0.5*dt)*a.
+// Returns a = F/m, formed after the Langevin term, for a caller that kicks again (k_cstep_boundary).
+template <bool THERMOSTAT, typename T>
+__device__ __forceinline__ T langevin_kick(T& v, T f, T m, T xi, T vc, T neg_gamma, T dt, T hdt) {
+  if (THERMOSTAT) v = add_rn(v, add_rn(mul_rn(mul_rn(neg_gamma, v), dt), mul_rn(xi, vc)));
+  const T acc = div_rn(f, m);
+  v = add_rn(v, mul_rn(hdt, acc));
+  return acc;
+}
+
+template <typename T>
 __global__ void __launch_bounds__(INTEG_THREADS)
-k_vv_first(int natoms, int lo, int cnt, unsigned long long* counters, float* __restrict__ pos,
-           float* __restrict__ vel, const float* __restrict__ forces, const float* __restrict__ masses,
-           float dt, float hdt) {
+k_vv_first(int natoms, int lo, int cnt, unsigned long long* counters, T* __restrict__ pos,
+           T* __restrict__ vel, const T* __restrict__ forces, const T* __restrict__ masses,
+           T dt, T hdt) {
   const int r = blockIdx.y;
   const int i = lo + blockIdx.x * blockDim.x + threadIdx.x;  // atoms [lo, lo+cnt) only
   if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) counters[1] += 1;  // Philox position of this step
   if (i >= lo + cnt) return;
-  const float m = masses[i];
+  const T m = masses[i];
   const size_t a = ((size_t)r * natoms + i) * 3;
 #pragma unroll
   for (int d = 0; d < 3; ++d) {
-    const float acc = div_rn(forces[a + d], m);
-    const float v = vel[a + d];
-    const float drift = add_rn(mul_rn(v, dt), mul_rn(mul_rn(mul_rn(0.5f, acc), dt), dt));
-    pos[a + d] = add_rn(pos[a + d], drift);
-    vel[a + d] = add_rn(v, mul_rn(hdt, acc));
+    const T acc = div_rn(forces[a + d], m);
+    T v = vel[a + d];
+    pos[a + d] = kick_drift(pos + a + d, v, acc, dt, hdt);
+    vel[a + d] = v;
   }
 }
 
@@ -54,11 +75,10 @@ k_vv_first_prepare(DeviceState S, float* __restrict__ pos, float* __restrict__ v
 #pragma unroll
   for (int d = 0; d < 3; ++d) {
     const float acc = div_rn(forces[a + d], m);
-    const float v = vel[a + d];
-    const float drift = add_rn(mul_rn(v, dt), mul_rn(mul_rn(mul_rn(0.5f, acc), dt), dt));
-    x[d] = add_rn(pos[a + d], drift);
+    float v = vel[a + d];
+    x[d] = kick_drift(pos + a + d, v, acc, dt, hdt);
     pos[a + d] = x[d];
-    vel[a + d] = add_rn(v, mul_rn(hdt, acc));
+    vel[a + d] = v;
   }
   prepare_atom(S, r, i, parity, x[0], x[1], x[2]);
 }
@@ -86,10 +106,9 @@ k_vv_first_push(int natoms, int lo, int cnt, unsigned long long* counters, const
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
       const float acc = div_rn(forces[a + d], m);
-      const float v = vel[a + d];
-      const float drift = add_rn(mul_rn(v, dt), mul_rn(mul_rn(mul_rn(0.5f, acc), dt), dt));
-      x[d] = add_rn(pos_in[a + d], drift);
-      vel[a + d] = add_rn(v, mul_rn(hdt, acc));
+      float v = vel[a + d];
+      x[d] = kick_drift(pos_in + a + d, v, acc, dt, hdt);
+      vel[a + d] = v;
     }
     for (int p = 0; p < pt.world; ++p) {
       float* dst = pt.pos[p] + a;
@@ -161,14 +180,39 @@ __device__ __forceinline__ void normal3(uint64_t seed, uint64_t step, uint64_t s
   out[1] = r0 * s;
   out[2] = r1 * cosf(two_pi * u3);
 }
+// the fp64 draws: two Philox4x32-10 blocks of the same stream (the second with the top counter bit set), 53-bit
+// uniforms, Box-Muller in fp64
+__device__ __forceinline__ double u53(unsigned hi, unsigned lo) {
+  return ((double)(((unsigned long long)(hi >> 5) << 26) | (lo >> 6)) + 0.5) * (1.0 / 9007199254740992.0);
+}
+__device__ __forceinline__ void normal3(uint64_t seed, uint64_t step, uint64_t slot, double out[3]) {
+  const uint2 key = make_uint2((unsigned)seed, (unsigned)(seed >> 32));
+  const uint4 u = philox4x32_10(make_uint4((unsigned)slot, (unsigned)(slot >> 32), (unsigned)step, (unsigned)(step >> 32)), key);
+  const uint4 w = philox4x32_10(make_uint4((unsigned)slot, (unsigned)(slot >> 32) | 0x80000000u, (unsigned)step, (unsigned)(step >> 32)), key);
+  const double two_pi = 6.283185307179586;
+  const double r0 = sqrt(-2.0 * log(u53(u.x, u.y))), r1 = sqrt(-2.0 * log(u53(w.x, w.y)));
+  double s, c;
+  sincos(two_pi * u53(u.z, u.w), &s, &c);
+  out[0] = r0 * c;
+  out[1] = r0 * s;
+  out[2] = r1 * cos(two_pi * u53(w.z, w.w));
+}
+// The Langevin noise of atom slot `slot` at `step`: the injected noise[3*slot..] if given, else the Philox draw.
+template <typename T>
+__device__ __forceinline__ void langevin_noise(const T* __restrict__ noise, uint64_t seed, uint64_t step, size_t slot, T xi[3]) {
+  if (noise) {
+    xi[0] = noise[3 * slot]; xi[1] = noise[3 * slot + 1]; xi[2] = noise[3 * slot + 2];
+  } else {
+    normal3(seed, step, slot, xi);
+  }
+}
 
-// [vel += ((-gamma*vel)*dt + xi*vcoeff)]  then  vel += (0.5*dt)*(F/m)
-// (integrator.py:72-74 then 67-69), optionally followed by the kinetic energy.
-template <bool THERMOSTAT, bool KINETIC, bool FOLD>
+// langevin_kick on every atom, optionally followed by the kinetic energy.
+template <typename T, bool THERMOSTAT, bool KINETIC, bool FOLD>
 __device__ __forceinline__ void vv_second_body(int natoms, int lo, int cnt, const unsigned long long* __restrict__ counters,
-                                               float* __restrict__ vel, const float* __restrict__ forces,
-                                               const float* __restrict__ masses, float dt, float hdt, float neg_gamma,
-                                               const float* __restrict__ vcoeff, const float* __restrict__ noise,
+                                               T* __restrict__ vel, const T* __restrict__ forces,
+                                               const T* __restrict__ masses, T dt, T hdt, T neg_gamma,
+                                               const T* __restrict__ vcoeff, const T* __restrict__ noise,
                                                uint64_t seed, uint64_t step_offset, double* __restrict__ ke,
                                                float* forces_rw, const double* __restrict__ scratch) {
   const int r = blockIdx.y;
@@ -176,24 +220,20 @@ __device__ __forceinline__ void vv_second_body(int natoms, int lo, int cnt, cons
   const uint64_t step = step_offset + counters[1];  // device-resident step count: graph replayable
   double ek = 0.0;
   if (i < lo + cnt) {
-    const float m = masses[i];
+    const T m = masses[i];
     const size_t slot = (size_t)r * natoms + i;
     const size_t a = slot * 3;
-    float xi[3] = {0.f, 0.f, 0.f};
-    float vc = 0.f;
+    T xi[3] = {T(0), T(0), T(0)};
+    T vc = T(0);
     if (THERMOSTAT) {
       vc = vcoeff[i];
-      if (noise) {
-        xi[0] = noise[a]; xi[1] = noise[a + 1]; xi[2] = noise[a + 2];
-      } else {
-        normal3(seed, step, slot, xi);
-      }
+      langevin_noise(noise, seed, step, slot, xi);
     }
-    float v2 = 0.f;
+    T v2 = T(0);
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
-      float f;
-      if (FOLD) {  // k_add_bonded's work (bonded.cuh): the bonded sums of the overlapped k_bonded_sum, rounded once
+      T f;
+      if constexpr (FOLD) {  // k_add_bonded's work (bonded.cuh): the bonded sums of the overlapped k_bonded_sum, rounded once
         f = forces_rw[a + d];
         const double sb = scratch[a + d];
         if (sb != 0.0) {
@@ -203,9 +243,8 @@ __device__ __forceinline__ void vv_second_body(int natoms, int lo, int cnt, cons
       } else {
         f = forces[a + d];
       }
-      float v = vel[a + d];
-      if (THERMOSTAT) v = add_rn(v, add_rn(mul_rn(mul_rn(neg_gamma, v), dt), mul_rn(xi[d], vc)));
-      v = add_rn(v, mul_rn(hdt, div_rn(f, m)));
+      T v = vel[a + d];
+      langevin_kick<THERMOSTAT>(v, f, m, xi[d], vc, neg_gamma, dt, hdt);
       vel[a + d] = v;
       v2 += v * v;
     }
@@ -217,15 +256,15 @@ __device__ __forceinline__ void vv_second_body(int natoms, int lo, int cnt, cons
   }
 }
 
-template <bool THERMOSTAT, bool KINETIC>
+template <typename T, bool THERMOSTAT, bool KINETIC>
 __global__ void __launch_bounds__(INTEG_THREADS)
 k_vv_second(int natoms, int lo, int cnt, const unsigned long long* __restrict__ counters,
-            float* __restrict__ vel, const float* __restrict__ forces,
-            const float* __restrict__ masses, float dt, float hdt, float neg_gamma,
-            const float* __restrict__ vcoeff, const float* __restrict__ noise, uint64_t seed,
+            T* __restrict__ vel, const T* __restrict__ forces,
+            const T* __restrict__ masses, T dt, T hdt, T neg_gamma,
+            const T* __restrict__ vcoeff, const T* __restrict__ noise, uint64_t seed,
             uint64_t step_offset, double* __restrict__ ke) {
-  vv_second_body<THERMOSTAT, KINETIC, false>(natoms, lo, cnt, counters, vel, forces, masses, dt, hdt, neg_gamma, vcoeff, noise, seed,
-                                             step_offset, ke, nullptr, nullptr);
+  vv_second_body<T, THERMOSTAT, KINETIC, false>(natoms, lo, cnt, counters, vel, forces, masses, dt, hdt, neg_gamma, vcoeff, noise,
+                                                seed, step_offset, ke, nullptr, nullptr);
 }
 
 // k_add_bonded + k_vv_second in one pass (tmd_md_steps with the bonded kernel overlapped on a second stream): the
@@ -237,19 +276,20 @@ k_vv_second_fold(int natoms, int lo, int cnt, const unsigned long long* __restri
                  const float* __restrict__ masses, float dt, float hdt, float neg_gamma,
                  const float* __restrict__ vcoeff, const float* __restrict__ noise, uint64_t seed,
                  uint64_t step_offset, double* __restrict__ ke, const double* __restrict__ scratch) {
-  vv_second_body<THERMOSTAT, KINETIC, true>(natoms, lo, cnt, counters, vel, nullptr, masses, dt, hdt, neg_gamma, vcoeff, noise, seed,
-                                            step_offset, ke, forces, scratch);
+  vv_second_body<float, THERMOSTAT, KINETIC, true>(natoms, lo, cnt, counters, vel, nullptr, masses, dt, hdt, neg_gamma, vcoeff,
+                                                   noise, seed, step_offset, ke, forces, scratch);
 }
 
+template <typename T>
 __global__ void __launch_bounds__(INTEG_THREADS)
-k_kinetic(int natoms, int lo, int cnt, const float* __restrict__ vel, const float* __restrict__ masses,
+k_kinetic(int natoms, int lo, int cnt, const T* __restrict__ vel, const T* __restrict__ masses,
           double* __restrict__ ke) {
   const int r = blockIdx.y;
   const int i = lo + blockIdx.x * blockDim.x + threadIdx.x;
   double ek = 0.0;
   if (i < lo + cnt) {
     const size_t a = ((size_t)r * natoms + i) * 3;
-    const float vx = vel[a], vy = vel[a + 1], vz = vel[a + 2];
+    const T vx = vel[a], vy = vel[a + 1], vz = vel[a + 2];
     ek = 0.5 * (double)masses[i] * (double)(vx * vx + vy * vy + vz * vz);
   }
   __shared__ double red[INTEG_THREADS / 32];

@@ -11,6 +11,7 @@
 #include <cmath>
 #include <string>
 #include <tuple>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -106,7 +107,7 @@ inline void launch_smem(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t 
 }
 
 // f(a, b) with a and b as std::integral_constant<bool, ...>: one launch line for the four <bool, bool> instantiations
-// of a kernel, as in with_bools(thermo, ke != nullptr, [&](auto th, auto e) { launch(k_vv_second<th, e>, ...); })
+// of a kernel, as in with_bools(thermo, ke != nullptr, [&](auto th, auto e) { launch(k_vv_second<float, th, e>, ...); })
 template <typename F>
 inline void with_bools(bool a, bool b, F&& f) {
   using T = std::true_type;
@@ -1548,12 +1549,12 @@ static inline dim3 owned_grid(const tmd_ctx* ctx, int threads) {
   return dim3((unsigned)((std::max(ctx->d.own_n, 1) + threads - 1) / threads), (unsigned)ctx->nrep);
 }
 
-// The kernels' bonded table (BondedTables or BondedTables64) from the context's sets, disabled terms emptied.
-template <typename Tables, typename Set>
-static Tables bonded_tables(const tmd_ctx* ctx, const Set& bonds, const Set& angles, const Set* torsions, const Set& pairs14,
-                            const Set& ub) {
+// The kernels' bonded table in precision P from the context's sets, disabled terms emptied.
+template <typename P>
+static BondedTablesT<P> bonded_tables(const tmd_ctx* ctx, const BondedSetT<P>& bonds, const BondedSetT<P>& angles,
+                                      const BondedSetT<P>* torsions, const BondedSetT<P>& pairs14, const BondedSetT<P>& ub) {
   const uint32_t bm = ctx->bonded_mask;
-  Tables T;
+  BondedTablesT<P> T;
   T.atom_ptr = ctx->bonded_atom_ptr;
   T.entries = ctx->bonded_entries;
   T.bonds = bonds;
@@ -1571,8 +1572,8 @@ static Tables bonded_tables(const tmd_ctx* ctx, const Set& bonds, const Set& ang
   return T;
 }
 // Where each (kind, term, slot) force sits in the per-term buffer of k_bonded_terms / k_bonded_sum.
-template <typename Tables>
-static TermLayout term_layout(const Tables& T) {
+template <typename P>
+static TermLayout term_layout(const BondedTablesT<P>& T) {
   TermLayout lay;
   const int cnt[BK_KINDS] = {T.bonds.n, T.angles.n, T.torsions[0].n, T.torsions[1].n, T.pairs14.n, T.cmap.n, T.ub.n};
   int nt = 0, ns = 0;
@@ -1686,13 +1687,14 @@ static int enqueue_forces_f64(tmd_ctx* ctx, const double* pos, double* forces, d
     TMD_CUDA(cudaMemsetAsync(forces, 0, (size_t)R * N * 3 * sizeof(double), st));
   }
   if (ctx->bonded_nentries > 0) {
-    const BondedTables64 T = bonded_tables<BondedTables64>(ctx, ctx->bonds64, ctx->angles64, ctx->torsions64, ctx->pairs1464, ctx->ub64);
+    const BondedTablesT<double> T = bonded_tables(ctx, ctx->bonds64, ctx->angles64, ctx->torsions64, ctx->pairs1464, ctx->ub64);
     const TermLayout lay = term_layout(T);
-    launch(k_bonded_terms_f64, dim3((std::max(lay.nterms, 1) + BONDED_THREADS - 1) / BONDED_THREADS, R), BONDED_THREADS, st, d, D, T, lay,
-           pos, energies, priv(ctx).term_forces);
-    TMD_LAUNCHED(ctx, "k_bonded_terms_f64");
-    launch(k_bonded_sum_f64, atoms_grid(ctx, BONDED_THREADS), BONDED_THREADS, st, d, T, lay, (const double*)priv(ctx).term_forces, forces);
-    TMD_LAUNCHED(ctx, "k_bonded_sum_f64");
+    launch(k_bonded_terms<double>, dim3((std::max(lay.nterms, 1) + BONDED_THREADS - 1) / BONDED_THREADS, R), BONDED_THREADS, st, d, T,
+           lay, D, pos, energies, priv(ctx).term_forces);
+    TMD_LAUNCHED(ctx, "k_bonded_terms");
+    launch(k_bonded_sum<double>, atoms_grid(ctx, BONDED_THREADS), BONDED_THREADS, st, d, T, lay, (const double*)priv(ctx).term_forces,
+           forces, (double*)nullptr);
+    TMD_LAUNCHED(ctx, "k_bonded_sum");
   }
   return TMD_OK;
 }
@@ -1703,7 +1705,7 @@ struct StepLink {
   bool prepared = false;                // in: the kernel before the force call did k_prepare's work,
   cudaGraphConditionalHandle cond = 0;  // and switches the rebuild's conditional node with this handle (when capturing)
   enum Tail { NONE, FOLD, DEFERRED } tail = NONE;  // out: what the force call left to the kernel after it
-  BondedTables T;                       // DEFERRED: k_bonded_vv_second evaluates these terms,
+  BondedTablesT<float> T;               // DEFERRED: k_bonded_vv_second evaluates these terms,
   const float* pos = nullptr;           // at these positions,
   double* energies = nullptr;           // and books their energies here
 };
@@ -1750,17 +1752,17 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
     TMD_CUDA(cudaEventRecord(pv.pme_join, pv.pme_side));
   }
 
-  BondedTables T;
+  BondedTablesT<float> T;
   const bool have_bonded = ctx->bonded_nentries > 0;
-  if (have_bonded) T = bonded_tables<BondedTables>(ctx, ctx->bonds, ctx->angles, ctx->torsions, ctx->pairs14, ctx->ub);
+  if (have_bonded) T = bonded_tables(ctx, ctx->bonds, ctx->angles, ctx->torsions, ctx->pairs14, ctx->ub);
   // bonded forces of the owned atoms: terms in parallel, then the fixed-order sum per atom (bonded.cuh)
   auto launch_bonded = [&](cudaStream_t bs, double* scratch) -> int {
     CtxPriv& pv = priv(ctx);
     const TermLayout lay = term_layout(T);
-    launch(k_bonded_terms, dim3((std::max(lay.nterms, 1) + BONDED_THREADS - 1) / BONDED_THREADS, R), BONDED_THREADS, bs, d, T, lay, ctx->q, pos,
-           energies, pv.term_forces);
+    launch(k_bonded_terms<float>, dim3((std::max(lay.nterms, 1) + BONDED_THREADS - 1) / BONDED_THREADS, R), BONDED_THREADS, bs, d, T, lay,
+           ctx->q, pos, energies, pv.term_forces);
     TMD_LAUNCHED(ctx, "k_bonded_terms");
-    launch(k_bonded_sum, owned_grid(ctx, BONDED_THREADS), BONDED_THREADS, bs, d, T, lay, pv.term_forces, forces, scratch);
+    launch(k_bonded_sum<float>, owned_grid(ctx, BONDED_THREADS), BONDED_THREADS, bs, d, T, lay, pv.term_forces, forces, scratch);
     TMD_LAUNCHED(ctx, "k_bonded_sum");
     return TMD_OK;
   };
@@ -1967,76 +1969,82 @@ static int enqueue_constrain_vel(tmd_ctx* ctx, const T* pos, T* vel, const T* ma
   return TMD_OK;
 }
 
-// link != nullptr: the force call of a step follows on this stream, and where can_prepare it finds its preparation
-// done.  boundary (the arguments of the tmd_md_steps call): k_cstep_boundary (fused.cuh) instead, which is also the
-// second half-kick of the step before, whose force call left its fold to this kernel.
-static int enqueue_vv_first(tmd_ctx* ctx, float* pos, float* vel, const float* forces, const float* masses,
-                            double dt, cudaStream_t st, StepLink* link = nullptr, const StepArgs* boundary = nullptr) {
-  if (link && can_prepare(ctx)) {
-    DeviceState dp = ctx->d;
-    if (int rc = capture_cond(ctx, st, dp)) return rc;
-    link->prepared = true;
-    link->cond = dp.cond;
-    if (boundary) {
-      const float fdt = (float)dt, hdt = (float)(0.5 * dt), ng = (float)(-boundary->gamma);
-      const bool thermo = (boundary->gamma >= 0.0) && boundary->vcoeff != nullptr;
-      launch(thermo ? k_cstep_boundary<true> : k_cstep_boundary<false>, atoms_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, dp,
-             pos, vel, masses, fdt, hdt, ng, boundary->vcoeff, boundary->seed, boundary->first_step, priv(ctx).bonded_scratch);
-      TMD_LAUNCHED(ctx, "k_cstep_boundary");
-      return TMD_OK;
-    }
-    launch(k_vv_first_prepare, atoms_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, dp, pos, vel, forces, masses, (float)dt,
-           (float)(0.5 * dt));
-    TMD_LAUNCHED(ctx, "k_vv_first_prepare");
-    return TMD_OK;
-  }
-  launch(k_vv_first, owned_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, 
-      ctx->natoms, ctx->d.own_lo, ctx->d.own_n, ctx->d.counters, pos, vel, forces, masses, (float)dt, (float)(0.5 * dt));
+// The first half-kick and drift of every owned atom.
+template <typename T>
+static int enqueue_vv_first(tmd_ctx* ctx, T* pos, T* vel, const T* forces, const T* masses, double dt, cudaStream_t st) {
+  launch(k_vv_first<T>, owned_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, ctx->natoms, ctx->d.own_lo, ctx->d.own_n, ctx->d.counters,
+         pos, vel, forces, masses, (T)dt, (T)(0.5 * dt));
   TMD_LAUNCHED(ctx, "k_vv_first");
   return TMD_OK;
 }
+// ... in an fp32 step (tmd_md_steps): link != nullptr: the force call of the step follows on this stream, and where
+// can_prepare it finds its preparation done.  boundary (the arguments of the call): k_cstep_boundary (fused.cuh)
+// instead, which is also the second half-kick of the step before, whose force call left its fold to this kernel.
+static int enqueue_vv_first(tmd_ctx* ctx, float* pos, float* vel, const float* forces, const float* masses, double dt,
+                            cudaStream_t st, StepLink* link, const StepArgs* boundary) {
+  if (!link || !can_prepare(ctx)) return enqueue_vv_first(ctx, pos, vel, forces, masses, dt, st);
+  DeviceState dp = ctx->d;
+  if (int rc = capture_cond(ctx, st, dp)) return rc;
+  link->prepared = true;
+  link->cond = dp.cond;
+  if (boundary) {
+    const float fdt = (float)dt, hdt = (float)(0.5 * dt), ng = (float)(-boundary->gamma);
+    const bool thermo = (boundary->gamma >= 0.0) && boundary->vcoeff != nullptr;
+    launch(thermo ? k_cstep_boundary<true> : k_cstep_boundary<false>, atoms_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, dp,
+           pos, vel, masses, fdt, hdt, ng, boundary->vcoeff, boundary->seed, boundary->first_step, priv(ctx).bonded_scratch);
+    TMD_LAUNCHED(ctx, "k_cstep_boundary");
+    return TMD_OK;
+  }
+  launch(k_vv_first_prepare, atoms_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, dp, pos, vel, forces, masses, (float)dt,
+         (float)(0.5 * dt));
+  TMD_LAUNCHED(ctx, "k_vv_first_prepare");
+  return TMD_OK;
+}
 
-// link: the second half-kick of a step also finishes what the step's force call left (StepLink::tail)
-static int enqueue_vv_second(tmd_ctx* ctx, float* vel, const float* forces, const float* masses, double dt,
-                             double gamma, const float* vcoeff, const float* noise, uint64_t seed,
-                             uint64_t step, double* ke, cudaStream_t st, const StepLink* link = nullptr) {
+// The Langevin kick and second half-kick of every owned atom; with ke, the kinetic energy after it.
+template <typename T>
+static int enqueue_vv_second(tmd_ctx* ctx, T* vel, const T* forces, const T* masses, double dt, double gamma, const T* vcoeff,
+                             const T* noise, uint64_t seed, uint64_t step, double* ke, cudaStream_t st) {
+  const bool thermo = (gamma >= 0.0) && vcoeff != nullptr;
+  if (ke) TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
+  with_bools(thermo, ke != nullptr, [&](auto th, auto e) {
+    launch(k_vv_second<T, th, e>, owned_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, ctx->natoms, ctx->d.own_lo, ctx->d.own_n,
+           ctx->d.counters, vel, forces, masses, (T)dt, (T)(0.5 * dt), (T)(-gamma), vcoeff, noise, seed, step, ke);
+  });
+  TMD_LAUNCHED(ctx, "k_vv_second");
+  return TMD_OK;
+}
+// ... in an fp32 step: it also finishes what the step's force call left (StepLink::tail)
+static int enqueue_vv_second(tmd_ctx* ctx, float* vel, const float* forces, const float* masses, double dt, double gamma,
+                             const float* vcoeff, const float* noise, uint64_t seed, uint64_t step, double* ke, cudaStream_t st,
+                             const StepLink& link) {
+  if (link.tail == StepLink::NONE) return enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step, ke, st);
   const bool thermo = (gamma >= 0.0) && vcoeff != nullptr;
   const dim3 g = owned_grid(ctx, INTEG_THREADS);
-  const int lo = ctx->d.own_lo, cnt = ctx->d.own_n;
-  const unsigned long long* ctr = ctx->d.counters;
   const float fdt = (float)dt, hdt = (float)(0.5 * dt), ng = (float)(-gamma);
   if (ke) TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
-  const StepLink::Tail tail = link ? link->tail : StepLink::NONE;
-  float* fw = const_cast<float*>(forces);  // (FOLD, DEFERRED: tmd_md_steps owns this buffer, the force call's output)
-  if (tail == StepLink::DEFERRED) {
+  float* fw = const_cast<float*>(forces);  // (tmd_md_steps owns this buffer, the force call's output)
+  if (link.tail == StepLink::DEFERRED) {
     with_bools(thermo, ke != nullptr, [&](auto th, auto e) {
-      launch(k_bonded_vv_second<th, e>, atoms_grid(ctx, BONDED_THREADS), BONDED_THREADS, st, ctx->d, link->T, ctx->q, link->pos, fw,
-             link->energies, vel, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke);
+      launch(k_bonded_vv_second<th, e>, atoms_grid(ctx, BONDED_THREADS), BONDED_THREADS, st, ctx->d, link.T, ctx->q, link.pos, fw,
+             link.energies, vel, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke);
     });
     TMD_LAUNCHED(ctx, "k_bonded_vv_second");
     return TMD_OK;
   }
   const double* sc = priv(ctx).bonded_scratch;
-  if (tail == StepLink::FOLD && ctx->d.cl.on) {  // cluster path: the pair forces come home from slot order on the way
+  if (ctx->d.cl.on) {  // cluster path: the pair forces come home from slot order on the way
     with_bools(thermo, ke != nullptr, [&](auto th, auto e) {
       launch(k_cvv_second_fold<th, e>, g, INTEG_THREADS, st, ctx->d, vel, fw, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke, sc);
     });
     TMD_LAUNCHED(ctx, "k_cvv_second_fold");
     return TMD_OK;
   }
-  if (tail == StepLink::FOLD) {
-    with_bools(thermo, ke != nullptr, [&](auto th, auto e) {
-      launch(k_vv_second_fold<th, e>, g, INTEG_THREADS, st, ctx->natoms, lo, cnt, ctr, vel, fw, masses, fdt, hdt, ng, vcoeff, noise,
-             seed, step, ke, sc);
-    });
-    TMD_LAUNCHED(ctx, "k_vv_second_fold");
-    return TMD_OK;
-  }
   with_bools(thermo, ke != nullptr, [&](auto th, auto e) {
-    launch(k_vv_second<th, e>, g, INTEG_THREADS, st, ctx->natoms, lo, cnt, ctr, vel, forces, masses, fdt, hdt, ng, vcoeff, noise,
-           seed, step, ke);
+    launch(k_vv_second_fold<th, e>, g, INTEG_THREADS, st, ctx->natoms, ctx->d.own_lo, ctx->d.own_n, ctx->d.counters, vel, fw, masses,
+           fdt, hdt, ng, vcoeff, noise, seed, step, ke, sc);
   });
-  TMD_LAUNCHED(ctx, "k_vv_second");
+  TMD_LAUNCHED(ctx, "k_vv_second_fold");
   return TMD_OK;
 }
 
@@ -2074,9 +2082,59 @@ static int enqueue_step(tmd_ctx* ctx, const StepArgs& a, const StepShape& shape,
   if (!shape.closes)  // the next step's k_cstep_boundary finishes this one: it adds the bonded sums
     return link.tail == StepLink::FOLD ? TMD_OK : fail(TMD_ERR_STATE, "tmd_md_steps: a step left open has no bonded fold for the next one");
   if ((rc = enqueue_vv_second(ctx, a.vel, a.forces, a.masses, a.dt, a.gamma, a.vcoeff, shape.noise, a.seed, a.first_step,
-                              shape.energies && !con ? a.ke : nullptr, st, &link)))
+                              shape.energies && !con ? a.ke : nullptr, st, link)))
     return rc;
   return con ? enqueue_constrain_vel(ctx, a.pos, a.vel, a.masses, shape.energies ? a.ke : nullptr, st) : TMD_OK;
+}
+
+// The standalone integrator entry points, both precisions: tmd_vv_first[_f64], tmd_vv_second[_f64],
+// tmd_kinetic_energy[_f64].  With constraints, the position and velocity projections follow the half-kicks.
+template <typename T>
+static constexpr int bits_of = (int)sizeof(T) * 8;
+
+template <typename T>
+static int vv_first(tmd_ctx* ctx, T* pos, T* vel, const T* forces, const T* masses, double dt, tmd_stream stream,
+                    const char* name) {
+  if (!ctx || !pos || !vel || !forces || !masses) return fail(TMD_ERR_ARG, std::string(name) + ": null pointer");
+  TMD_PRECISION(ctx, bits_of<T>, name)
+  DeviceGuard guard(ctx->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool con = has_constraints(ctx);
+  int rc;
+  if (con && (rc = con_save_ref(ctx, pos, st))) return rc;
+  if ((rc = enqueue_vv_first(ctx, pos, vel, forces, masses, dt, st))) return rc;
+  if (!con) return TMD_OK;
+  priv(ctx).con_pos = pos;
+  return enqueue_constrain_pos(ctx, pos, static_cast<const T*>(priv(ctx).con_ref), vel, masses, dt, st);
+}
+
+template <typename T>
+static int vv_second(tmd_ctx* ctx, T* vel, const T* forces, const T* masses, double dt, double gamma, const T* vcoeff,
+                     const T* noise, uint64_t seed, uint64_t step_index, double* ke, tmd_stream stream, const char* name) {
+  if (!ctx || !vel || !forces || !masses) return fail(TMD_ERR_ARG, std::string(name) + ": null pointer");
+  TMD_PRECISION(ctx, bits_of<T>, name)
+  DeviceGuard guard(ctx->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool con = has_constraints(ctx);
+  if (con && !priv(ctx).con_pos)
+    return fail(TMD_ERR_STATE, std::string(name) + ": constraints are set but tmd_vv_first" + (bits_of<T> == 64 ? "_f64" : "") +
+                                   " has not run");
+  int rc;
+  if ((rc = enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step_index, con ? nullptr : ke, st)))
+    return rc;
+  return con ? enqueue_constrain_vel(ctx, static_cast<const T*>(priv(ctx).con_pos), vel, masses, ke, st) : TMD_OK;
+}
+
+template <typename T>
+static int kinetic_energy(tmd_ctx* ctx, const T* vel, const T* masses, double* ke, tmd_stream stream, const char* name) {
+  if (!ctx || !vel || !masses || !ke) return fail(TMD_ERR_ARG, std::string(name) + ": null pointer");
+  TMD_PRECISION(ctx, bits_of<T>, name)
+  DeviceGuard guard(ctx->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
+  launch(k_kinetic<T>, owned_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, ctx->natoms, ctx->d.own_lo, ctx->d.own_n, vel, masses, ke);
+  TMD_LAUNCHED(ctx, "k_kinetic");
+  return TMD_OK;
 }
 
 extern "C" {
@@ -2093,40 +2151,29 @@ int tmd_forces(tmd_ctx* ctx, const float* pos, float* forces, double* energies, 
 
 int tmd_vv_first(tmd_ctx* ctx, float* pos, float* vel, const float* forces, const float* masses, double dt,
                  tmd_stream stream) {
-  if (!ctx || !pos || !vel || !forces || !masses) return fail(TMD_ERR_ARG, "tmd_vv_first: null pointer");
-  TMD_PRECISION(ctx, 32, "tmd_vv_first")
-  DeviceGuard guard(ctx->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (!has_constraints(ctx)) return enqueue_vv_first(ctx, pos, vel, forces, masses, dt, st);
-  int rc;
-  if ((rc = con_save_ref(ctx, pos, st)) || (rc = enqueue_vv_first(ctx, pos, vel, forces, masses, dt, st))) return rc;
-  priv(ctx).con_pos = pos;
-  return enqueue_constrain_pos(ctx, pos, static_cast<const float*>(priv(ctx).con_ref), vel, masses, dt, st);
+  return vv_first(ctx, pos, vel, forces, masses, dt, stream, "tmd_vv_first");
+}
+int tmd_vv_first_f64(tmd_ctx* ctx, double* pos, double* vel, const double* forces, const double* masses, double dt,
+                     tmd_stream stream) {
+  return vv_first(ctx, pos, vel, forces, masses, dt, stream, "tmd_vv_first_f64");
 }
 
 int tmd_vv_second(tmd_ctx* ctx, float* vel, const float* forces, const float* masses, double dt, double gamma,
                   const float* vcoeff, const float* noise, uint64_t seed, uint64_t step_index, double* ke,
                   tmd_stream stream) {
-  if (!ctx || !vel || !forces || !masses) return fail(TMD_ERR_ARG, "tmd_vv_second: null pointer");
-  TMD_PRECISION(ctx, 32, "tmd_vv_second")
-  DeviceGuard guard(ctx->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (!has_constraints(ctx)) return enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step_index, ke, st);
-  if (!priv(ctx).con_pos) return fail(TMD_ERR_STATE, "tmd_vv_second: constraints are set but tmd_vv_first has not run");
-  int rc;
-  if ((rc = enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step_index, nullptr, st))) return rc;
-  return enqueue_constrain_vel(ctx, static_cast<const float*>(priv(ctx).con_pos), vel, masses, ke, st);
+  return vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step_index, ke, stream, "tmd_vv_second");
+}
+int tmd_vv_second_f64(tmd_ctx* ctx, double* vel, const double* forces, const double* masses, double dt, double gamma,
+                      const double* vcoeff, const double* noise, uint64_t seed, uint64_t step_index, double* ke,
+                      tmd_stream stream) {
+  return vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step_index, ke, stream, "tmd_vv_second_f64");
 }
 
 int tmd_kinetic_energy(tmd_ctx* ctx, const float* vel, const float* masses, double* ke, tmd_stream stream) {
-  if (!ctx || !vel || !masses || !ke) return fail(TMD_ERR_ARG, "tmd_kinetic_energy: null pointer");
-  TMD_PRECISION(ctx, 32, "tmd_kinetic_energy")
-  DeviceGuard guard(ctx->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
-  launch(k_kinetic, owned_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, ctx->natoms, ctx->d.own_lo, ctx->d.own_n, vel, masses, ke);
-  TMD_LAUNCHED(ctx, "k_kinetic");
-  return TMD_OK;
+  return kinetic_energy(ctx, vel, masses, ke, stream, "tmd_kinetic_energy");
+}
+int tmd_kinetic_energy_f64(tmd_ctx* ctx, const double* vel, const double* masses, double* ke, tmd_stream stream) {
+  return kinetic_energy(ctx, vel, masses, ke, stream, "tmd_kinetic_energy_f64");
 }
 
 int tmd_md_steps(tmd_ctx* ctx, int niter, float* pos, float* vel, float* forces, const float* masses,
@@ -2251,66 +2298,6 @@ int tmd_forces_f64(tmd_ctx* ctx, const double* pos, double* forces, double* ener
   return enqueue_forces_f64(ctx, pos, forces, energies, st);
 }
 
-static void enqueue_vv_first_f64(tmd_ctx* ctx, double* pos, double* vel, const double* forces, const double* masses, double dt,
-                                 cudaStream_t st) {
-  launch(k_vv_first_f64, atoms_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, ctx->natoms, ctx->d.counters, pos, vel, forces, masses,
-         dt, 0.5 * dt);
-}
-static void enqueue_vv_second_f64(tmd_ctx* ctx, double* vel, const double* forces, const double* masses, double dt, double gamma,
-                                  const double* vcoeff, const double* noise, uint64_t seed, uint64_t step, double* ke,
-                                  cudaStream_t st) {
-  const bool thermo = (gamma >= 0.0) && vcoeff != nullptr;
-  const dim3 g = atoms_grid(ctx, INTEG_THREADS);
-  const int n = ctx->natoms;
-  const unsigned long long* ctr = ctx->d.counters;
-  with_bools(thermo, ke != nullptr, [&](auto th, auto e) {
-    launch(k_vv_second_f64<th, e>, g, INTEG_THREADS, st, n, ctr, vel, forces, masses, dt, 0.5 * dt, -gamma, vcoeff, noise, seed, step, ke);
-  });
-}
-
-int tmd_vv_first_f64(tmd_ctx* ctx, double* pos, double* vel, const double* forces, const double* masses, double dt,
-                     tmd_stream stream) {
-  if (!ctx || !pos || !vel || !forces || !masses) return fail(TMD_ERR_ARG, "tmd_vv_first_f64: null pointer");
-  TMD_PRECISION(ctx, 64, "tmd_vv_first_f64")
-  DeviceGuard guard(ctx->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  const bool con = has_constraints(ctx);
-  int rc;
-  if (con && (rc = con_save_ref(ctx, pos, st))) return rc;
-  enqueue_vv_first_f64(ctx, pos, vel, forces, masses, dt, st);
-  TMD_LAUNCHED(ctx, "k_vv_first_f64");
-  if (!con) return TMD_OK;
-  priv(ctx).con_pos = pos;
-  return enqueue_constrain_pos(ctx, pos, static_cast<const double*>(priv(ctx).con_ref), vel, masses, dt, st);
-}
-
-int tmd_vv_second_f64(tmd_ctx* ctx, double* vel, const double* forces, const double* masses, double dt, double gamma,
-                      const double* vcoeff, const double* noise, uint64_t seed, uint64_t step_index, double* ke,
-                      tmd_stream stream) {
-  if (!ctx || !vel || !forces || !masses) return fail(TMD_ERR_ARG, "tmd_vv_second_f64: null pointer");
-  TMD_PRECISION(ctx, 64, "tmd_vv_second_f64")
-  DeviceGuard guard(ctx->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  const bool con = has_constraints(ctx);
-  if (con && !priv(ctx).con_pos) return fail(TMD_ERR_STATE, "tmd_vv_second_f64: constraints are set but tmd_vv_first_f64 has not run");
-  if (ke && !con) TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
-  enqueue_vv_second_f64(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step_index, con ? nullptr : ke, st);
-  TMD_LAUNCHED(ctx, "k_vv_second_f64");
-  if (con) return enqueue_constrain_vel(ctx, static_cast<const double*>(priv(ctx).con_pos), vel, masses, ke, st);
-  return TMD_OK;
-}
-
-int tmd_kinetic_energy_f64(tmd_ctx* ctx, const double* vel, const double* masses, double* ke, tmd_stream stream) {
-  if (!ctx || !vel || !masses || !ke) return fail(TMD_ERR_ARG, "tmd_kinetic_energy_f64: null pointer");
-  TMD_PRECISION(ctx, 64, "tmd_kinetic_energy_f64")
-  DeviceGuard guard(ctx->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
-  launch(k_kinetic_f64, atoms_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, ctx->natoms, vel, masses, ke);
-  TMD_LAUNCHED(ctx, "k_kinetic_f64");
-  return TMD_OK;
-}
-
 int tmd_md_steps_f64(tmd_ctx* ctx, int niter, double* pos, double* vel, double* forces, const double* masses, double dt,
                      double gamma, const double* vcoeff, const double* noise, uint64_t seed, uint64_t first_step,
                      double* energies, double* ke, tmd_stream stream) {
@@ -2327,15 +2314,12 @@ int tmd_md_steps_f64(tmd_ctx* ctx, int niter, double* pos, double* vel, double* 
   for (int it = 0; it < niter; ++it) {
     const bool last = (it == niter - 1);
     if (con && (rc = con_save_ref(ctx, pos, st))) return rc;
-    enqueue_vv_first_f64(ctx, pos, vel, forces, masses, dt, st);
-    TMD_LAUNCHED(ctx, "k_vv_first_f64");
+    if ((rc = enqueue_vv_first(ctx, pos, vel, forces, masses, dt, st))) return rc;
     if (con && (rc = enqueue_constrain_pos(ctx, pos, cref, vel, masses, dt, st))) return rc;
     if ((rc = enqueue_forces_f64(ctx, pos, forces, last ? energies : nullptr, st))) return rc;
-    double* ke2 = last && !con ? ke : nullptr;
-    if (ke2) TMD_CUDA(cudaMemsetAsync(ke2, 0, (size_t)ctx->nrep * sizeof(double), st));
-    enqueue_vv_second_f64(ctx, vel, forces, masses, dt, gamma, vcoeff, noise ? noise + it * per_step : nullptr, seed, first_step,
-                          ke2, st);
-    TMD_LAUNCHED(ctx, "k_vv_second_f64");
+    if ((rc = enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise ? noise + it * per_step : nullptr,
+                                seed, first_step, last && !con ? ke : nullptr, st)))
+      return rc;
     if (con && (rc = enqueue_constrain_vel(ctx, pos, vel, masses, last ? ke : nullptr, st))) return rc;
   }
   return TMD_OK;
