@@ -379,6 +379,33 @@ int tmd_scale_molecules_f64(tmd_ctx* ctx, double* pos_dev, const double* scale_d
 int64_t tmd_step_captures(tmd_ctx* ctx);
 int tmd_rewind_noise(tmd_ctx* ctx, int nsteps, tmd_stream stream);
 
+/* ---- parallel tempering: per-replica temperatures and replica exchange (library version >= 107) ----
+ *
+ * tmd_set_temperature_ladder(ctx, ntemps, temperatures_host, ladder_dev) gives the replicas a ladder
+ * of ntemps = R temperatures (K, positive) and the caller-owned (R,) int32 device array ladder_dev,
+ * a permutation of 0..R-1: ladder_dev[r] is the temperature index of replica r.  While it is set,
+ * the vcoeff argument of tmd_md_steps[_f64] and tmd_vv_second[_f64] is an (R, N, 1) table, and
+ * replica r takes its Langevin noise scale from row ladder_dev[r].  ntemps = 0 clears it (vcoeff is
+ * one (N,1) row again).  The context keeps the address: setting a new one makes the captured step
+ * graphs recapture once, rewriting its contents costs nothing.  [sync: the ladder is checked]
+ * TMD_ERR_UNSUPPORTED on a decomposed or peer-to-peer context.
+ *
+ * tmd_replica_exchange[_f64](ctx, energies_dev, stride, nterms, seed, attempt, vel_dev, counts_dev,
+ * stream) runs exchange attempt `attempt` in stream order, with no read-back: U_r = sum over
+ * t < nterms of energies_dev[r*stride + t] (fp64, in term order); the pairs of temperature slots
+ * (k, k+1) with k = attempt (mod 2), held by replicas i and j, swap with probability
+ * min(1, exp((1/kT_k - 1/kT_{k+1}) (U_i - U_j))), the uniform being u53 of Philox4x32-10 on the
+ * counter (k, 0x40000000, attempt lo, attempt hi) under the key seed (csrc/remd.cuh); a replica
+ * whose temperature changed has its velocities scaled by sqrt(T_new / T_old).  counts_dev (R-1, 2)
+ * int64 accumulates the attempts and acceptances of each pair of slots.  TMD_ERR_ARG for R < 2 or
+ * R > 1024, TMD_ERR_STATE without a ladder, TMD_ERR_UNSUPPORTED on a decomposed or peer-to-peer
+ * context. */
+int tmd_set_temperature_ladder(tmd_ctx* ctx, int ntemps, const double* temperatures_host, int32_t* ladder_dev);
+int tmd_replica_exchange(tmd_ctx* ctx, const double* energies_dev, int stride, int nterms, uint64_t seed, uint64_t attempt,
+                         float* vel_dev, int64_t* counts_dev, tmd_stream stream);
+int tmd_replica_exchange_f64(tmd_ctx* ctx, const double* energies_dev, int stride, int nterms, uint64_t seed,
+                             uint64_t attempt, double* vel_dev, int64_t* counts_dev, tmd_stream stream);
+
 /* ---- inspection ------------------------------------------------------------ */
 
 /* The reference's neighbour list for one replica: every non-excluded pair

@@ -13,5 +13,6 @@ from .parameters import TopologyParameters  # noqa: F401
 from .constraints import Constraints  # noqa: F401
 from .wrapper import Wrapper  # noqa: F401
 from .barostat import MonteCarloBarostat  # noqa: F401
+from .replica_exchange import ReplicaExchange  # noqa: F401
 
 __version__ = "0.1.0"

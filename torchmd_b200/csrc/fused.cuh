@@ -16,7 +16,8 @@ __global__ void __launch_bounds__(BONDED_THREADS)
 k_bonded_vv_second(DeviceState S, BondedTablesT<float> T, const float* __restrict__ q_scaled, const float* __restrict__ pos,
                    float* __restrict__ forces, double* __restrict__ energies, float* __restrict__ vel,
                    const float* __restrict__ masses, float dt, float hdt, float neg_gamma, const float* __restrict__ vcoeff,
-                   const float* __restrict__ noise, uint64_t seed, uint64_t step_offset, double* __restrict__ ke) {
+                   const float* __restrict__ noise, uint64_t seed, uint64_t step_offset, double* __restrict__ ke,
+                   const int* __restrict__ ladder) {
   const int r = blockIdx.y;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;  // whole system (cluster path)
   const uint64_t step = step_offset + S.counters[1];
@@ -33,7 +34,7 @@ k_bonded_vv_second(DeviceState S, BondedTablesT<float> T, const float* __restric
     float xi[3] = {0.f, 0.f, 0.f};
     float vc = 0.f;
     if (THERMOSTAT) {
-      vc = vcoeff[i];
+      vc = langevin_scale(vcoeff, ladder, r, S.natoms, i);
       langevin_noise(noise, seed, step, slot, xi);
     }
     float v2 = 0.f;
@@ -72,7 +73,8 @@ template <bool THERMOSTAT, bool KINETIC>
 __global__ void __launch_bounds__(INTEG_THREADS)
 k_cvv_second_fold(DeviceState S, float* __restrict__ vel, float* __restrict__ forces, const float* __restrict__ masses, float dt,
                   float hdt, float neg_gamma, const float* __restrict__ vcoeff, const float* __restrict__ noise, uint64_t seed,
-                  uint64_t step_offset, double* __restrict__ ke, const double* __restrict__ scratch) {
+                  uint64_t step_offset, double* __restrict__ ke, const double* __restrict__ scratch,
+                  const int* __restrict__ ladder) {
   const int r = blockIdx.y;
   const int i = S.own_lo + blockIdx.x * blockDim.x + threadIdx.x;
   const uint64_t step = step_offset + S.counters[1];
@@ -86,7 +88,7 @@ k_cvv_second_fold(DeviceState S, float* __restrict__ vel, float* __restrict__ fo
     float xi[3] = {0.f, 0.f, 0.f};
     float vc = 0.f;
     if (THERMOSTAT) {
-      vc = vcoeff[i];
+      vc = langevin_scale(vcoeff, ladder, r, S.natoms, i);
       langevin_noise(noise, seed, step, slot, xi);
     }
     float v2 = 0.f;
@@ -118,7 +120,7 @@ template <bool THERMOSTAT>
 __global__ void __launch_bounds__(INTEG_THREADS)
 k_cstep_boundary(DeviceState S, float* __restrict__ pos, float* __restrict__ vel, const float* __restrict__ masses, float dt,
                  float hdt, float neg_gamma, const float* __restrict__ vcoeff, uint64_t seed, uint64_t step_offset,
-                 const double* __restrict__ scratch) {
+                 const double* __restrict__ scratch, const int* __restrict__ ladder) {
   const int parity = (int)(S.counters[0] & 1ull);
   const int r = blockIdx.y;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;  // whole system
@@ -134,7 +136,7 @@ k_cstep_boundary(DeviceState S, float* __restrict__ pos, float* __restrict__ vel
   float xi[3] = {0.f, 0.f, 0.f};
   float vc = 0.f;
   if (THERMOSTAT) {
-    vc = vcoeff[i];
+    vc = langevin_scale(vcoeff, ladder, r, S.natoms, i);
     normal3(seed, step, slot, xi);
   }
   float x[3];

@@ -207,6 +207,13 @@ __device__ __forceinline__ void langevin_noise(const T* __restrict__ noise, uint
   }
 }
 
+// The Langevin noise scale of atom i of replica r: vcoeff is one (N,1) row, or with a temperature ladder (remd.cuh) an
+// (R,N,1) table of which replica r reads row ladder[r].  The branch is uniform (a kernel argument).
+template <typename T>
+__device__ __forceinline__ T langevin_scale(const T* __restrict__ vcoeff, const int* __restrict__ ladder, int r, int natoms, int i) {
+  return ladder ? vcoeff[(size_t)ladder[r] * natoms + i] : vcoeff[i];
+}
+
 // langevin_kick on every atom, optionally followed by the kinetic energy.
 template <typename T, bool THERMOSTAT, bool KINETIC, bool FOLD>
 __device__ __forceinline__ void vv_second_body(int natoms, int lo, int cnt, const unsigned long long* __restrict__ counters,
@@ -214,7 +221,8 @@ __device__ __forceinline__ void vv_second_body(int natoms, int lo, int cnt, cons
                                                const T* __restrict__ masses, T dt, T hdt, T neg_gamma,
                                                const T* __restrict__ vcoeff, const T* __restrict__ noise,
                                                uint64_t seed, uint64_t step_offset, double* __restrict__ ke,
-                                               float* forces_rw, const double* __restrict__ scratch) {
+                                               float* forces_rw, const double* __restrict__ scratch,
+                                               const int* __restrict__ ladder) {
   const int r = blockIdx.y;
   const int i = lo + blockIdx.x * blockDim.x + threadIdx.x;
   const uint64_t step = step_offset + counters[1];  // device-resident step count: graph replayable
@@ -226,7 +234,7 @@ __device__ __forceinline__ void vv_second_body(int natoms, int lo, int cnt, cons
     T xi[3] = {T(0), T(0), T(0)};
     T vc = T(0);
     if (THERMOSTAT) {
-      vc = vcoeff[i];
+      vc = langevin_scale(vcoeff, ladder, r, natoms, i);
       langevin_noise(noise, seed, step, slot, xi);
     }
     T v2 = T(0);
@@ -262,9 +270,9 @@ k_vv_second(int natoms, int lo, int cnt, const unsigned long long* __restrict__ 
             T* __restrict__ vel, const T* __restrict__ forces,
             const T* __restrict__ masses, T dt, T hdt, T neg_gamma,
             const T* __restrict__ vcoeff, const T* __restrict__ noise, uint64_t seed,
-            uint64_t step_offset, double* __restrict__ ke) {
+            uint64_t step_offset, double* __restrict__ ke, const int* __restrict__ ladder) {
   vv_second_body<T, THERMOSTAT, KINETIC, false>(natoms, lo, cnt, counters, vel, forces, masses, dt, hdt, neg_gamma, vcoeff, noise,
-                                                seed, step_offset, ke, nullptr, nullptr);
+                                                seed, step_offset, ke, nullptr, nullptr, ladder);
 }
 
 // k_add_bonded + k_vv_second in one pass (tmd_md_steps with the bonded kernel overlapped on a second stream): the
@@ -275,9 +283,10 @@ k_vv_second_fold(int natoms, int lo, int cnt, const unsigned long long* __restri
                  float* __restrict__ vel, float* __restrict__ forces,
                  const float* __restrict__ masses, float dt, float hdt, float neg_gamma,
                  const float* __restrict__ vcoeff, const float* __restrict__ noise, uint64_t seed,
-                 uint64_t step_offset, double* __restrict__ ke, const double* __restrict__ scratch) {
+                 uint64_t step_offset, double* __restrict__ ke, const double* __restrict__ scratch,
+                 const int* __restrict__ ladder) {
   vv_second_body<float, THERMOSTAT, KINETIC, true>(natoms, lo, cnt, counters, vel, nullptr, masses, dt, hdt, neg_gamma, vcoeff,
-                                                   noise, seed, step_offset, ke, forces, scratch);
+                                                   noise, seed, step_offset, ke, forces, scratch, ladder);
 }
 
 template <typename T>

@@ -27,6 +27,7 @@
 #include "constrain.cuh"
 #include "pme.cuh"
 #include "barostat.cuh"
+#include "remd.cuh"
 
 using namespace tmd;
 
@@ -177,6 +178,7 @@ struct StepArgs {
   double dt, gamma;
   uint64_t seed, first_step;
   double *energies, *ke;
+  const int* ladder;  // temperature index of each replica (tmd_set_temperature_ladder), or null: part of the step-graph key
 };
 
 struct CtxPriv {
@@ -253,6 +255,10 @@ struct CtxPriv {
   int mol_n = 0;
   int *mol_ptr = nullptr, *mol_atoms = nullptr, *mol_parent = nullptr;
   double* mol_u = nullptr;
+  // tmd_set_temperature_ladder (remd.cuh): the caller's (R,) ladder, the temperatures, the velocity factors of an exchange
+  const int* ladder = nullptr;
+  double* remd_T = nullptr;
+  double* remd_factor = nullptr;
 };
 
 }  // namespace
@@ -336,7 +342,7 @@ const char* tmd_last_error(void) { return g_err.c_str(); }
 #if defined(TMD_SIMT_HOST)
 int tmd_version(void) { return -100; }  // host SIMT interpreter build (tests/simt): torchmd_b200/_lib.py refuses it
 #else
-int tmd_version(void) { return 106; }  // 101: the "precision: double" entry points (tmd_set_precision, *_f64); 102: constraints; 103: PME; 104: box rescale + molecule scaling; 105: CMAP; 106: Urey-Bradley
+int tmd_version(void) { return 107; }  // 101: the "precision: double" entry points (tmd_set_precision, *_f64); 102: constraints; 103: PME; 104: box rescale + molecule scaling; 105: CMAP; 106: Urey-Bradley; 107: temperature ladder + replica exchange
 #endif
 
 int tmd_create(tmd_ctx** out, int device, int natoms, int nreplicas) {
@@ -425,7 +431,8 @@ int tmd_destroy(tmd_ctx* ctx) {
   {
     CtxPriv& p = priv(ctx);
     for (void* b : {(void*)p.pme_q, (void*)p.pme_L, (void*)p.pme_tw, (void*)p.pme_econst, (void*)p.pme_qgrid, p.pme_cgrid, p.pme_infl,
-                    (void*)p.pme_mod, (void*)p.box_dev, (void*)p.mol_ptr, (void*)p.mol_atoms, (void*)p.mol_parent, (void*)p.mol_u})
+                    (void*)p.pme_mod, (void*)p.box_dev, (void*)p.mol_ptr, (void*)p.mol_atoms, (void*)p.mol_parent, (void*)p.mol_u,
+                    (void*)p.remd_T, (void*)p.remd_factor})
       if (b) cudaFree(b);
     if (p.pme_side) cudaStreamDestroy(p.pme_side);
     if (p.pme_fork) cudaEventDestroy(p.pme_fork);
@@ -1991,7 +1998,8 @@ static int enqueue_vv_first(tmd_ctx* ctx, float* pos, float* vel, const float* f
     const float fdt = (float)dt, hdt = (float)(0.5 * dt), ng = (float)(-boundary->gamma);
     const bool thermo = (boundary->gamma >= 0.0) && boundary->vcoeff != nullptr;
     launch(thermo ? k_cstep_boundary<true> : k_cstep_boundary<false>, atoms_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, dp,
-           pos, vel, masses, fdt, hdt, ng, boundary->vcoeff, boundary->seed, boundary->first_step, priv(ctx).bonded_scratch);
+           pos, vel, masses, fdt, hdt, ng, boundary->vcoeff, boundary->seed, boundary->first_step, priv(ctx).bonded_scratch,
+           boundary->ladder);
     TMD_LAUNCHED(ctx, "k_cstep_boundary");
     return TMD_OK;
   }
@@ -2001,15 +2009,16 @@ static int enqueue_vv_first(tmd_ctx* ctx, float* pos, float* vel, const float* f
   return TMD_OK;
 }
 
-// The Langevin kick and second half-kick of every owned atom; with ke, the kinetic energy after it.
+// The Langevin kick and second half-kick of every owned atom; with ke, the kinetic energy after it.  ladder: replica r
+// takes its noise scale from row ladder[r] of vcoeff (remd.cuh), or null.
 template <typename T>
 static int enqueue_vv_second(tmd_ctx* ctx, T* vel, const T* forces, const T* masses, double dt, double gamma, const T* vcoeff,
-                             const T* noise, uint64_t seed, uint64_t step, double* ke, cudaStream_t st) {
+                             const T* noise, uint64_t seed, uint64_t step, double* ke, cudaStream_t st, const int* ladder) {
   const bool thermo = (gamma >= 0.0) && vcoeff != nullptr;
   if (ke) TMD_CUDA(cudaMemsetAsync(ke, 0, (size_t)ctx->nrep * sizeof(double), st));
   with_bools(thermo, ke != nullptr, [&](auto th, auto e) {
     launch(k_vv_second<T, th, e>, owned_grid(ctx, INTEG_THREADS), INTEG_THREADS, st, ctx->natoms, ctx->d.own_lo, ctx->d.own_n,
-           ctx->d.counters, vel, forces, masses, (T)dt, (T)(0.5 * dt), (T)(-gamma), vcoeff, noise, seed, step, ke);
+           ctx->d.counters, vel, forces, masses, (T)dt, (T)(0.5 * dt), (T)(-gamma), vcoeff, noise, seed, step, ke, ladder);
   });
   TMD_LAUNCHED(ctx, "k_vv_second");
   return TMD_OK;
@@ -2017,8 +2026,9 @@ static int enqueue_vv_second(tmd_ctx* ctx, T* vel, const T* forces, const T* mas
 // ... in an fp32 step: it also finishes what the step's force call left (StepLink::tail)
 static int enqueue_vv_second(tmd_ctx* ctx, float* vel, const float* forces, const float* masses, double dt, double gamma,
                              const float* vcoeff, const float* noise, uint64_t seed, uint64_t step, double* ke, cudaStream_t st,
-                             const StepLink& link) {
-  if (link.tail == StepLink::NONE) return enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step, ke, st);
+                             const int* ladder, const StepLink& link) {
+  if (link.tail == StepLink::NONE)
+    return enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step, ke, st, ladder);
   const bool thermo = (gamma >= 0.0) && vcoeff != nullptr;
   const dim3 g = owned_grid(ctx, INTEG_THREADS);
   const float fdt = (float)dt, hdt = (float)(0.5 * dt), ng = (float)(-gamma);
@@ -2027,7 +2037,7 @@ static int enqueue_vv_second(tmd_ctx* ctx, float* vel, const float* forces, cons
   if (link.tail == StepLink::DEFERRED) {
     with_bools(thermo, ke != nullptr, [&](auto th, auto e) {
       launch(k_bonded_vv_second<th, e>, atoms_grid(ctx, BONDED_THREADS), BONDED_THREADS, st, ctx->d, link.T, ctx->q, link.pos, fw,
-             link.energies, vel, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke);
+             link.energies, vel, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke, ladder);
     });
     TMD_LAUNCHED(ctx, "k_bonded_vv_second");
     return TMD_OK;
@@ -2035,14 +2045,15 @@ static int enqueue_vv_second(tmd_ctx* ctx, float* vel, const float* forces, cons
   const double* sc = priv(ctx).bonded_scratch;
   if (ctx->d.cl.on) {  // cluster path: the pair forces come home from slot order on the way
     with_bools(thermo, ke != nullptr, [&](auto th, auto e) {
-      launch(k_cvv_second_fold<th, e>, g, INTEG_THREADS, st, ctx->d, vel, fw, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke, sc);
+      launch(k_cvv_second_fold<th, e>, g, INTEG_THREADS, st, ctx->d, vel, fw, masses, fdt, hdt, ng, vcoeff, noise, seed, step, ke, sc,
+             ladder);
     });
     TMD_LAUNCHED(ctx, "k_cvv_second_fold");
     return TMD_OK;
   }
   with_bools(thermo, ke != nullptr, [&](auto th, auto e) {
     launch(k_vv_second_fold<th, e>, g, INTEG_THREADS, st, ctx->natoms, ctx->d.own_lo, ctx->d.own_n, ctx->d.counters, vel, fw, masses,
-           fdt, hdt, ng, vcoeff, noise, seed, step, ke, sc);
+           fdt, hdt, ng, vcoeff, noise, seed, step, ke, sc, ladder);
   });
   TMD_LAUNCHED(ctx, "k_vv_second_fold");
   return TMD_OK;
@@ -2082,7 +2093,7 @@ static int enqueue_step(tmd_ctx* ctx, const StepArgs& a, const StepShape& shape,
   if (!shape.closes)  // the next step's k_cstep_boundary finishes this one: it adds the bonded sums
     return link.tail == StepLink::FOLD ? TMD_OK : fail(TMD_ERR_STATE, "tmd_md_steps: a step left open has no bonded fold for the next one");
   if ((rc = enqueue_vv_second(ctx, a.vel, a.forces, a.masses, a.dt, a.gamma, a.vcoeff, shape.noise, a.seed, a.first_step,
-                              shape.energies && !con ? a.ke : nullptr, st, link)))
+                              shape.energies && !con ? a.ke : nullptr, st, a.ladder, link)))
     return rc;
   return con ? enqueue_constrain_vel(ctx, a.pos, a.vel, a.masses, shape.energies ? a.ke : nullptr, st) : TMD_OK;
 }
@@ -2120,7 +2131,8 @@ static int vv_second(tmd_ctx* ctx, T* vel, const T* forces, const T* masses, dou
     return fail(TMD_ERR_STATE, std::string(name) + ": constraints are set but tmd_vv_first" + (bits_of<T> == 64 ? "_f64" : "") +
                                    " has not run");
   int rc;
-  if ((rc = enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step_index, con ? nullptr : ke, st)))
+  if ((rc = enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise, seed, step_index, con ? nullptr : ke, st,
+                              priv(ctx).ladder)))
     return rc;
   return con ? enqueue_constrain_vel(ctx, static_cast<const T*>(priv(ctx).con_pos), vel, masses, ke, st) : TMD_OK;
 }
@@ -2195,7 +2207,7 @@ int tmd_md_steps(tmd_ctx* ctx, int niter, float* pos, float* vel, float* forces,
   const bool fuse = pv.fuse_step && pv.fuse_prepare && ctx->d.cl.on && ctx->d.own_all && ctx->pair_mask && !noise &&
                     ctx->bonded_nentries > 0 && pv.side != nullptr && niter >= 2 && !con;
   if (con) pv.con_pos = pos;
-  const StepArgs args{pos, vel, forces, masses, vcoeff, dt, gamma, seed, first_step, energies, ke};
+  const StepArgs args{pos, vel, forces, masses, vcoeff, dt, gamma, seed, first_step, energies, ke, pv.ladder};
   if (pv.use_graph && !noise && !pv.profiling && niter > 0) {
     // One MD step captured once (with and without the energy outputs) and replayed: one graph
     // launch per step, the rebuild kernels inside a conditional node.  Everything that changes
@@ -2318,7 +2330,7 @@ int tmd_md_steps_f64(tmd_ctx* ctx, int niter, double* pos, double* vel, double* 
     if (con && (rc = enqueue_constrain_pos(ctx, pos, cref, vel, masses, dt, st))) return rc;
     if ((rc = enqueue_forces_f64(ctx, pos, forces, last ? energies : nullptr, st))) return rc;
     if ((rc = enqueue_vv_second(ctx, vel, forces, masses, dt, gamma, vcoeff, noise ? noise + it * per_step : nullptr,
-                                seed, first_step, last && !con ? ke : nullptr, st)))
+                                seed, first_step, last && !con ? ke : nullptr, st, priv(ctx).ladder)))
       return rc;
     if (con && (rc = enqueue_constrain_vel(ctx, pos, vel, masses, last ? ke : nullptr, st))) return rc;
   }
@@ -2605,6 +2617,74 @@ int tmd_rewind_noise(tmd_ctx* ctx, int nsteps, tmd_stream stream) {
   position -= (unsigned long long)nsteps;
   TMD_CUDA(cudaMemcpy(ctx->d.counters + 1, &position, sizeof(position), cudaMemcpyHostToDevice));
   return TMD_OK;
+}
+
+// ---- parallel tempering: per-replica temperatures and replica exchanges (remd.cuh) ---------------
+static bool decomposed(tmd_ctx* ctx) { return ctx->dd_base || !ctx->d.own_all; }
+
+int tmd_set_temperature_ladder(tmd_ctx* ctx, int ntemps, const double* temperatures_host, int32_t* ladder_dev) {
+  if (!ctx || ntemps < 0) return fail(TMD_ERR_ARG, "tmd_set_temperature_ladder: bad arguments");
+  CtxPriv& pv = priv(ctx);
+  if (ntemps == 0) {
+    pv.ladder = nullptr;
+    return TMD_OK;
+  }
+  const int R = ctx->nrep;
+  if (ntemps != R || !temperatures_host || !ladder_dev)
+    return fail(TMD_ERR_ARG, "tmd_set_temperature_ladder: one temperature per replica and a ladder array are needed");
+  if (decomposed(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_temperature_ladder: decomposed and peer-to-peer runs have one temperature");
+  for (int k = 0; k < R; ++k)
+    if (!(temperatures_host[k] > 0.0) || !(temperatures_host[k] < INFINITY))
+      return fail(TMD_ERR_ARG, "tmd_set_temperature_ladder: temperatures must be positive and finite");
+  DeviceGuard guard(ctx->device);
+  // the kernels index vcoeff rows with the ladder: check it is a permutation (the setter may synchronise)
+  std::vector<int32_t> lad(R);
+  TMD_CUDA(cudaDeviceSynchronize());
+  TMD_CUDA(cudaMemcpy(lad.data(), ladder_dev, (size_t)R * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  std::vector<char> seen(R, 0);
+  for (int r = 0; r < R; ++r) {
+    if (lad[r] < 0 || lad[r] >= R || seen[lad[r]]) return fail(TMD_ERR_ARG, "tmd_set_temperature_ladder: the ladder is not a permutation of 0..R-1");
+    seen[lad[r]] = 1;
+  }
+  int rc;
+  if (!pv.remd_T && (rc = device_alloc(&pv.remd_T, (size_t)R))) return rc;
+  if (!pv.remd_factor && (rc = device_alloc(&pv.remd_factor, (size_t)R))) return rc;
+  TMD_CUDA(cudaMemcpy(pv.remd_T, temperatures_host, (size_t)R * sizeof(double), cudaMemcpyHostToDevice));
+  pv.ladder = ladder_dev;
+  return TMD_OK;
+}
+
+extern "C++" {
+template <typename T>
+static int replica_exchange(tmd_ctx* ctx, const double* energies, int stride, int nterms, uint64_t seed, uint64_t attempt, T* vel,
+                            int64_t* counts, tmd_stream stream, const char* name) {
+  const std::string who = std::string(name) + ": ";
+  if (!ctx || !energies || !vel || !counts || nterms < 1 || stride < nterms) return fail(TMD_ERR_ARG, who + "bad arguments");
+  TMD_PRECISION(ctx, bits_of<T>, name)
+  CtxPriv& pv = priv(ctx);
+  const int R = ctx->nrep;
+  if (decomposed(ctx)) return fail(TMD_ERR_UNSUPPORTED, who + "decomposed and peer-to-peer runs do not exchange replicas");
+  if (R < 2 || R > REMD_MAX_REPLICAS) return fail(TMD_ERR_ARG, who + "an exchange needs 2 to 1024 replicas");
+  if (!pv.ladder) return fail(TMD_ERR_STATE, who + "call tmd_set_temperature_ladder first");
+  DeviceGuard guard(ctx->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  launch(k_remd_exchange, 1, (R + 31) / 32 * 32, st, R, energies, stride, nterms, (const double*)pv.remd_T, const_cast<int*>(pv.ladder),
+         seed, attempt, pv.remd_factor, reinterpret_cast<long long*>(counts));
+  TMD_LAUNCHED(ctx, "k_remd_exchange");
+  launch(k_remd_scale<T>, dim3((ctx->natoms * 3 + INTEG_THREADS - 1) / INTEG_THREADS, R), INTEG_THREADS, st, ctx->natoms, vel,
+         (const double*)pv.remd_factor);
+  TMD_LAUNCHED(ctx, "k_remd_scale");
+  return TMD_OK;
+}
+}  // extern "C++"
+
+int tmd_replica_exchange(tmd_ctx* ctx, const double* energies_dev, int stride, int nterms, uint64_t seed, uint64_t attempt,
+                         float* vel_dev, int64_t* counts_dev, tmd_stream stream) {
+  return replica_exchange(ctx, energies_dev, stride, nterms, seed, attempt, vel_dev, counts_dev, stream, "tmd_replica_exchange");
+}
+int tmd_replica_exchange_f64(tmd_ctx* ctx, const double* energies_dev, int stride, int nterms, uint64_t seed, uint64_t attempt,
+                             double* vel_dev, int64_t* counts_dev, tmd_stream stream) {
+  return replica_exchange(ctx, energies_dev, stride, nterms, seed, attempt, vel_dev, counts_dev, stream, "tmd_replica_exchange_f64");
 }
 
 int tmd_set_molecules(tmd_ctx* ctx, int nmol, const int32_t* ptr, const int32_t* atoms, const int32_t* parent) {

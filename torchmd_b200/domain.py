@@ -33,6 +33,7 @@ Opt-in until validated on a multi-GPU H100 machine.
 import ctypes as C
 import os
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -91,6 +92,8 @@ class DecomposedIntegrator:
             raise NotImplementedError("the Monte Carlo barostat runs on one GPU: use Integrator(..., barostat=...)")
         if constraints is not None:
             raise NotImplementedError("constraints run on one GPU: use Integrator(..., constraints=...)")
+        if T is not None and np.ndim(T) > 0:
+            raise NotImplementedError("per-replica temperatures run on one GPU: use Integrator(..., T=[...])")
         if getattr(forces, "pme", False):
             raise NotImplementedError("particle-mesh Ewald runs on one GPU: use Integrator with Forces(..., pme=True)")
         if system.pos.dtype == torch.float64:

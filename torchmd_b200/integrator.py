@@ -17,6 +17,12 @@ counts the constrained degrees of freedom out (``Constraints.ndof``); ``Ekin`` s
 where the step index reaches a multiple of its ``frequency``, and each such chunk is followed by one Monte Carlo volume
 move per replica, which writes the accepted box into ``systems.box``.  The returned energies describe the state after
 the move.
+
+``T`` is one temperature or a sequence of one per replica.  With a sequence, ``vcoeff`` is an (R, N, 1) table, one row
+per temperature (row k is the ``vcoeff`` of a run at ``T[k]``), and replica r takes its noise from row ``ladder[r]`` of
+an (R,) int32 device ladder, the identity unless ``replica_exchange`` (a ``torchmd_b200.ReplicaExchange``) swaps
+temperatures between replicas.  Exchange attempts follow every ``frequency``-th step, like the barostat's moves; when
+one ends a call, the returned ``Ekin`` and ``T`` describe the scaled velocities.
 """
 import ctypes as C
 
@@ -45,8 +51,19 @@ def kinetic_energy(masses, vel, batch=None):
     return out
 
 
+def _is_sequence(T):
+    return isinstance(T, (list, tuple, np.ndarray, torch.Tensor)) and np.ndim(T) > 0
+
+
 def maxwell_boltzmann(masses, T, replicas=1):
-    """Velocities ~ sqrt(kB T / m) N(0,1) per replica (integrator.py:46-54)."""
+    """Velocities ~ sqrt(kB T / m) N(0,1) per replica (integrator.py:46-54).  ``T``: one temperature, or a sequence of
+    ``replicas`` temperatures, replica r drawn at ``T[r]``."""
+    if _is_sequence(T):
+        temps = [float(t) for t in T]
+        if len(temps) != replicas:
+            raise ValueError(f"maxwell_boltzmann: {len(temps)} temperatures for {replicas} replicas")
+        draws = [torch.sqrt(t * BOLTZMAN / masses) * torch.randn((len(masses), 3)).type_as(masses) for t in temps]
+        return torch.stack(draws, dim=0)
     scale = torch.sqrt(T * BOLTZMAN / masses)
     draws = [scale * torch.randn((len(masses), 3)).type_as(masses) for _ in range(replicas)]
     return torch.stack(draws, dim=0)
@@ -58,7 +75,26 @@ def kinetic_to_temp(Ekin, natoms):
 
 
 class Integrator:
-    def __init__(self, systems, forces, timestep, device, gamma=None, T=None, batch=None, constraints=None, barostat=None):
+    def __init__(self, systems, forces, timestep, device, gamma=None, T=None, batch=None, constraints=None, barostat=None,
+                 replica_exchange=None):
+        nrep = systems.pos.shape[0]
+        self.temperatures = None  # the ladder's temperatures (a sequence T), or None
+        if _is_sequence(T):
+            self.temperatures = [float(t) for t in T]
+            if len(self.temperatures) != nrep:
+                raise ValueError(f"T has {len(self.temperatures)} temperatures for {nrep} replicas")
+            if not all(t > 0.0 and np.isfinite(t) for t in self.temperatures):
+                raise ValueError("the temperatures must be positive and finite")
+            T = self.temperatures
+        if replica_exchange is not None:
+            if gamma is None or T is None:
+                raise RuntimeError("replica exchange needs a thermostat: give the Integrator gamma and a list of temperatures")
+            if self.temperatures is None:
+                raise ValueError("replica exchange needs one temperature per replica: give T as a sequence")
+            if barostat is not None:
+                raise RuntimeError("replica exchange cannot run with a barostat: the barostat's kT is one temperature")
+        if barostat is not None and self.temperatures is not None:
+            raise RuntimeError("MonteCarloBarostat runs at one temperature: give T as a scalar")
         self.dt = timestep / TIMEFACTOR
         self.systems = systems
         self.forces = forces
@@ -74,7 +110,12 @@ class Integrator:
             self.masses = (
                 forces.par.masses.clone().detach().to(device=device, dtype=systems.pos.dtype).view(-1, 1)
             )
-        if T:
+        self._ladder = None  # (R,) int32 device ladder of a sequence T: replica r reads vcoeff row _ladder[r]
+        if self.temperatures is not None:
+            # one row per temperature, each the expression of the scalar case
+            self.vcoeff = torch.stack([torch.sqrt(2.0 * gamma / self.masses * BOLTZMAN * t * self.dt) for t in self.temperatures]).to(device)
+            self._ladder = torch.arange(nrep, dtype=torch.int32, device=systems.pos.device)
+        elif T:
             self.vcoeff = torch.sqrt(2.0 * gamma / self.masses * BOLTZMAN * T * self.dt).to(device)
         self.batch = batch
         if batch is not None:
@@ -102,6 +143,9 @@ class Integrator:
             if not bool((diag > 0).all()) or bool((off != 0).any()):
                 raise RuntimeError("MonteCarloBarostat needs a periodic orthorhombic box on every replica")
             barostat._bind(self)
+        self.replica_exchange = replica_exchange
+        if replica_exchange is not None:
+            replica_exchange._bind(self)
 
     def __del__(self):
         try:
@@ -160,6 +204,14 @@ class Integrator:
             else:
                 _lib.check(_lib.lib().tmd_set_constraints(ctx, 0, None, None, 0, None, None, None))
             ctx._tmd_constraints = self.constraints
+        # the temperature ladder, shared the same way: an integrator with one temperature must not run on another's
+        if getattr(ctx, "_tmd_ladder", None) is not self._ladder:
+            if self._ladder is not None:
+                temps = np.ascontiguousarray(self.temperatures, dtype=np.float64)
+                _lib.check(_lib.lib().tmd_set_temperature_ladder(ctx, len(temps), temps.ctypes.data, self._ladder.data_ptr()))
+            else:
+                _lib.check(_lib.lib().tmd_set_temperature_ladder(ctx, 0, None, None))
+            ctx._tmd_ladder = self._ladder
         return ctx
 
     def step(self, niter=1, noise=None):
@@ -189,6 +241,8 @@ class Integrator:
             _lib.check(getattr(L, "tmd_constrain" + sfx)(ctx, s.pos.data_ptr(), s.vel.data_ptr(), self.masses.data_ptr(), stream))
             self._projected = True
         native = isinstance(self.forces, Forces) and not self.forces.external
+        rex = self.replica_exchange
+        exchanged = False  # the call ended with an exchange: the kinetic energy is that of the scaled velocities
         pot = None
         if native and niter > 0:
             f = self.forces
@@ -198,11 +252,12 @@ class Integrator:
                 f._exact_gradient = False
             ene = self._out[1]
             bar = self.barostat
+            period = bar.frequency if bar is not None else (rex.frequency if rex is not None else None)
             done = 0
             while done < niter:
-                # with a barostat the steps run in chunks that end where a move is due
-                n = niter - done if bar is None else min(niter - done, bar.frequency - self._step_index % bar.frequency)
-                chunk_noise = noise[done:done + n] if noise is not None and bar is not None else noise
+                # with a barostat or replica exchange the steps run in chunks that end where a move is due
+                n = niter - done if period is None else min(niter - done, period - self._step_index % period)
+                chunk_noise = noise[done:done + n] if noise is not None and period is not None else noise
                 # A neighbour list that outgrows its reserved capacity inside the fused call invalidates the call (the
                 # kernels truncate, the library grows the capacity at the stats() check).  The state is three small
                 # tensors: keep a copy and run the call again from it instead of giving up.  Everything else a step reads
@@ -234,8 +289,12 @@ class Integrator:
                 self._step_index += n
                 done += n
                 pot = None
+                exchanged = False
                 if bar is not None and self._step_index % bar.frequency == 0:
                     pot = [float(e) for e in bar.attempt(ctx, ene)]
+                if rex is not None and self._step_index % rex.frequency == 0:  # (after the chunk's overflow check)
+                    rex.attempt(ctx, ene, _lib.NUM_ENERGIES, _lib.NUM_ENERGIES)
+                    exchanged = True
             if pot is None:
                 pot = f._format(ene, None, s.pos.dtype, False, True)
         else:
@@ -253,10 +312,16 @@ class Integrator:
                     )
                 )
                 self._step_index += 1
+                exchanged = rex is not None and self._step_index % rex.frequency == 0
+                if exchanged:  # from this step's potential energies, the external term included
+                    pot_dev = torch.as_tensor(np.asarray(pot, dtype=np.float64).reshape(nrep, 1)).to(s.pos.device)
+                    rex.attempt(ctx, pot_dev, 1, 1)
             if niter <= 0:
                 _lib.check(getattr(L, "tmd_kinetic_energy" + sfx)(ctx, s.vel.data_ptr(), self.masses.data_ptr(), ke.data_ptr(), stream))
             elif self.constraints is not None:  # (the fused path learns of a failed constraint group from f.stats())
                 _lib.check(L.tmd_get_stats(ctx, C.byref(_lib.Stats()), stream))
+        if exchanged:
+            _lib.check(getattr(L, "tmd_kinetic_energy" + sfx)(ctx, s.vel.data_ptr(), self.masses.data_ptr(), ke.data_ptr(), stream))
 
         if self.batch is None:
             Ekin = ke.cpu().numpy().astype(np.float64 if f64 else np.float32)  # the state's dtype, like integrator.py:122-125
