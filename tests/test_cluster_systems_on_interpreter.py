@@ -6,6 +6,7 @@ import pytest
 import torch
 
 from test_mirrors_on_interpreter import _install
+from torchmd_b200._lib import PAIR_CLUSTER, PAIR_ROWS_FX2
 
 
 @pytest.fixture
@@ -37,7 +38,7 @@ def test_atom_types_on_the_cluster_kernel(hostsim, T):
 
     spec = G.retyped(G.tiled_water(2), T, seed=T)
     forces, pos, box, F, E, kern = G.run(spec)
-    assert kern == G.CLUSTER, kern
+    assert kern == PAIR_CLUSTER, kern
     G.check_fp32(spec, forces, pos, box, F, E, f"{T} types", tol=G.RETYPED_TOL)
 
 
@@ -59,5 +60,5 @@ def test_dilute_gas_at_a_long_cutoff_takes_the_full_rows(hostsim):
     par = testsystems.argon_parameters(sysd, precision=torch.float64)
     spec = G._spec_of(par, sysd["coords"], sysd["box"], ["lj"], dict(cutoff=16.0, switch_dist=14.0), sysd["name"])
     forces, pos, box, F, E, kern = G.run(spec)
-    assert kern == G.FULL_ROWS, kern
+    assert kern == PAIR_ROWS_FX2, kern
     G.check_fp32(spec, forces, pos, box, F, E, "argon gas at cutoff 16")

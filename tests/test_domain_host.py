@@ -12,6 +12,7 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 from conftest import ROOT
+from torchmd_b200._lib import PAIR_CLUSTER
 
 
 def test_ranges_cover_every_atom_once():
@@ -407,7 +408,7 @@ def _worker_integrator_cluster(rank, world, port, out):
     e1 = single.step(8)
     e2 = dec.step(8)
     lo, hi = dec.dec.lo, dec.dec.hi
-    ok = ok and _lib.lib().tmd_pair_kernel(f2._ctx) == 4 and _lib.lib().tmd_pair_kernel(f1._ctx) == 4
+    ok = ok and _lib.lib().tmd_pair_kernel(f2._ctx) == PAIR_CLUSTER and _lib.lib().tmd_pair_kernel(f1._ctx) == PAIR_CLUSTER
     ok = ok and (s1.pos - s2.pos).abs().max().item() < 5e-5 and (s1.vel[:, lo:hi] - s2.vel[:, lo:hi]).abs().max().item() < 5e-4
     ok = ok and abs(e1[1][0] - e2[1][0]) <= 1e-5 * abs(e1[1][0]) + 2e-2
     ok = ok and f2.stats()["rebuilds"] >= 2

@@ -6,6 +6,7 @@ import torch
 
 from oracle import refmd
 from test_simt_cluster import CFG, TERMS, _compute, _oracle, tiled_water
+from torchmd_b200._lib import PAIR_CLUSTER, PAIR_ROWS_FX, PAIR_ROWS_FX2
 
 pytestmark = [pytest.mark.gpu]
 DEV = "cuda:0"
@@ -27,7 +28,7 @@ def test_gpu_cluster_periodic_water(thrown):
         sh = rng.integers(-thrown, thrown + 1, size=coords.shape).astype(np.float32)
         coords = coords + sh * (rng.random(len(coords)) < 0.3)[:, None] * np.float32(L)
     system, forces, e = _compute(sysd, coords, None, dev=DEV)
-    assert _L().tmd_pair_kernel(forces._ctx) == 4, "the cluster kernel did not run"
+    assert _L().tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER, "the cluster kernel did not run"
     f64, e_ref, pairs_ref = _oracle(sysd, system)
     pairs = forces.neighbour_pairs(system.pos, system.box).cpu().numpy()
     assert pairs.shape == pairs_ref.shape and np.array_equal(pairs, pairs_ref.astype(np.int32))
@@ -54,7 +55,7 @@ def test_gpu_cluster_band_pairs():
         shift = (coords[a].astype(np.float64) + u * float(r)) - coords[b].astype(np.float64)
         coords[b : b + 3] = (coords[b : b + 3].astype(np.float64) + shift).astype(np.float32)
     system, forces, e = _compute(sysd, coords, None, dev=DEV)
-    assert _L().tmd_pair_kernel(forces._ctx) == 4
+    assert _L().tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER
     f64, e_ref, pairs_ref = _oracle(sysd, system)
     assert np.array_equal(forces.neighbour_pairs(system.pos, system.box).cpu().numpy(), pairs_ref.astype(np.int32))
     scale = max(1.0, f64.abs().max().item() / 100.0)
@@ -82,12 +83,12 @@ def test_gpu_cluster_headline_size_against_the_sampled_oracle():
     eq = Integrator(system, full, 1.0, DEV, gamma=10.0, T=300.0)
     for _ in range(6):
         eq.step(niter=100)  # lattice start -> liquid (as bench.py does)
-    assert _L().tmd_pair_kernel(full._ctx) == 4
+    assert _L().tmd_pair_kernel(full._ctx) == PAIR_CLUSTER
     pair_terms = ["lj", "electrostatics"]
     forces = Forces(par, terms=pair_terms, **cfg)
     F = torch.empty_like(system.pos)
     forces.compute(system.pos, system.box, F)
-    assert _L().tmd_pair_kernel(forces._ctx) == 4
+    assert _L().tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER
     pairs = forces.neighbour_pairs(system.pos, system.box).cpu().numpy()
     atoms = sorted(np.random.default_rng(7).choice(n, 600, replace=False).tolist())
     par64 = testsystems.water_parameters(sysd, precision=torch.float64)
@@ -125,7 +126,7 @@ def test_gpu_cluster_md_follows_the_full_list_trajectory(monkeypatch):
         integ = Integrator(system, forces, 1.0, DEV, gamma=None, T=None)
         ekin, pot, temp = integ.step(niter=40)
         st = forces.stats()
-        assert _L().tmd_pair_kernel(forces._ctx) == (4 if cluster == "1" else 2)
+        assert _L().tmd_pair_kernel(forces._ctx) == (PAIR_CLUSTER if cluster == "1" else PAIR_ROWS_FX2)
         assert st["rebuilds"] >= 3, st
         out.append((system.pos.clone(), system.vel.clone(), ekin, pot))
     # (40 steps; stiff O-H bonds amplify the 5e-5 force differences of the two summation orders)
@@ -141,13 +142,13 @@ def test_gpu_cluster_capacity_growth_and_fallback(monkeypatch):
     coords = np.array(sysd["coords"], dtype=np.float32)
     monkeypatch.setenv("TMD_B200_CLUSTER_ECAP", "64")
     system, forces, e = _compute(sysd, coords, None, dev=DEV)
-    assert _L().tmd_pair_kernel(forces._ctx) == 4
+    assert _L().tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER
     f64, e_ref, _ = _oracle(sysd, system)
     assert (system.forces.cpu().double() - f64).abs().max().item() < 1e-4
     monkeypatch.delenv("TMD_B200_CLUSTER_ECAP")
     lat = testsystems.water_box(1500, seed=0)
     system, forces, e = _compute(lat, np.array(lat["coords"], dtype=np.float32), None, dev=DEV)
-    assert _L().tmd_pair_kernel(forces._ctx) in (1, 2), "expected the fall-back to the full rows"
+    assert _L().tmd_pair_kernel(forces._ctx) in (PAIR_ROWS_FX, PAIR_ROWS_FX2), "expected the fall-back to the full rows"
     f64, e_ref, pairs_ref = _oracle(lat, system)
     assert (system.forces.cpu().double() - f64).abs().max().item() < 1e-4 * max(1.0, f64.abs().max().item() / 100.0)
     assert np.array_equal(forces.neighbour_pairs(system.pos, system.box).cpu().numpy(), pairs_ref.astype(np.int32))

@@ -26,10 +26,10 @@ import torch
 
 from oracle import refmd
 from test_simt_cluster import tiled_water
+from torchmd_b200._lib import PAIR_CLUSTER, PAIR_EWALD_CLUSTER, PAIR_F64, PAIR_ROWS_FX2
 
 pytestmark = [pytest.mark.gpu]
 DEV = "cuda:0"
-CLUSTER, FULL_ROWS, FP64, CLUSTER_EW = 4, 2, 5, 10  # tmd_pair_kernel ids (include/tmd_b200.h)
 TABLES = {"bonds": "bond_params", "angles": "angle_params", "dihedrals": "dihedral_params", "impropers": "improper_params",
           "pairs14": "nonbonded_14_params"}
 BONDED = ("bonds", "angles", "dihedrals", "impropers", "1-4")
@@ -306,7 +306,7 @@ def protein_rf(variant, t=2):
     spec = protein(t)
     coords, boxes = configurations(spec, variant)
     forces, pos, box, F, E, kern = run(spec, coords, boxes)
-    assert kern == CLUSTER, (variant, kern)
+    assert kern == PAIR_CLUSTER, (variant, kern)
     return check_fp32(spec, forces, pos, box, F, E, f"ala2 x{t}^3 RF {variant}, kernel {kern}")
 
 
@@ -314,7 +314,7 @@ def protein_pme(variant, t=2):
     spec = protein(t)
     coords, boxes = configurations(spec, variant)
     forces, pos, box, F, E, kern = run(spec, coords, boxes, pme=True)
-    assert kern == CLUSTER_EW, (variant, kern)
+    assert kern == PAIR_EWALD_CLUSTER, (variant, kern)
     return check_pme(spec, forces, pos, boxes, F, E, f"ala2 x{t}^3 PME {variant}, kernel {kern}")
 
 
@@ -333,7 +333,7 @@ def test_solvated_protein_charmm_like_cutoff():
     spec = protein(3)
     over = dict(cutoff=12.0, switch_dist=10.0)
     forces, pos, box, F, E, kern = run(spec, **over)
-    assert kern == CLUSTER, kern
+    assert kern == PAIR_CLUSTER, kern
     _, e_b = check_sampled(spec, forces, pos, box, F, f"ala2 x3^3 cutoff 12, kernel {kern}", **over)
     for k in ("bonds", "angles", "dihedrals", "impropers"):
         assert abs(E[0][k] - e_b[k]) <= 1e-5 * abs(e_b[k]) + 2e-3, (k, E[0][k], e_b[k])
@@ -371,7 +371,7 @@ def protein_md_follows_the_full_rows(monkeypatch, nsteps=40, t=2):
         integ = Integrator(system, forces, 1.0, DEV, gamma=None, T=None)
         ekin, pot, _ = integ.step(niter=nsteps)
         kern = _L().tmd_pair_kernel(forces._ctx)
-        assert kern == (CLUSTER if cluster == "1" else FULL_ROWS), (cluster, kern)
+        assert kern == (PAIR_CLUSTER if cluster == "1" else PAIR_ROWS_FX2), (cluster, kern)
         assert forces.stats()["rebuilds"] >= 3, forces.stats()
         fresh_epot_matches(forces, system, pot, cluster)
         out.append((system.pos.clone(), system.vel.clone(), ekin, pot))
@@ -396,7 +396,7 @@ def protein_hbonds_2fs(nsteps=200, chunk=20, t=2):
     groups = OC.groups_of(con)
     for _ in range(nsteps // chunk):
         _, pot, _ = integ.step(chunk)
-        assert _L().tmd_pair_kernel(forces._ctx) == CLUSTER
+        assert _L().tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER
         box = torch.diagonal(system.box, dim1=-2, dim2=-1).cpu().double().numpy()
         er, ev = OC.residuals(system.pos.cpu().double().numpy(), system.vel.cpu().double().numpy(), groups, box)
         assert er <= 2 * float(np.spacing(np.float32(system.pos.abs().max().item()))), er
@@ -419,13 +419,13 @@ def types_on_every_path(monkeypatch, T, t=2):
     spec = retyped(tiled_water(t), T, seed=T)
     what = f"water x{t}^3, {T} types"
     forces, pos, box, F, E, kern = run(spec)
-    assert kern == CLUSTER, (T, kern)
+    assert kern == PAIR_CLUSTER, (T, kern)
     Fo, Eo, pairs = oracle(spec, pos, box, torch.float32)
     results = {kern: (forces, F, E)}
     monkeypatch.setenv("TMD_B200_CLUSTER", "0")
     forces2, _, _, F2, E2, kern2 = run(spec)
     monkeypatch.delenv("TMD_B200_CLUSTER")
-    assert kern2 == FULL_ROWS, (T, kern2)
+    assert kern2 == PAIR_ROWS_FX2, (T, kern2)
     results[kern2] = (forces2, F2, E2)
     for k, (fo, Fk, Ek) in results.items():
         got = fo.neighbour_pairs(pos, box).cpu().numpy()
@@ -436,10 +436,10 @@ def types_on_every_path(monkeypatch, T, t=2):
         for term in spec["terms"]:
             assert abs(Ek[0][term] - Eo[0][term]) <= 1e-5 * abs(Eo[0][term]) + 2e-3, (T, k, term, Ek[0][term], Eo[0][term])
     forces, pos, box, F, E, kern = run(spec, pme=True)
-    assert kern == CLUSTER_EW, (T, kern)
+    assert kern == PAIR_EWALD_CLUSTER, (T, kern)
     check_pme(spec, forces, pos, spec["box"][None], F, E, f"{what} PME, kernel {kern}")
     forces, pos, box, F, E, kern = run(spec, dtype=torch.float64)
-    assert kern == FP64, (T, kern)
+    assert kern == PAIR_F64, (T, kern)
     check_fp64(spec, pos, box, F, E, f"{what} fp64, kernel {kern}")
 
 
@@ -456,7 +456,7 @@ def more_than_128_types_are_refused(dtype, t=2):
         run(retyped(tiled_water(t), 129), dtype=dtype)
     spec = retyped(tiled_water(t), 128)
     forces, pos, box, F, E, kern = run(spec, dtype=dtype)
-    assert kern == (CLUSTER if dtype == torch.float32 else FP64), kern
+    assert kern == (PAIR_CLUSTER if dtype == torch.float32 else PAIR_F64), kern
     assert torch.isfinite(F).all()
     if dtype == torch.float32:
         check_fp32(spec, forces, pos, box, F, E, "128 types after a refused context", tol=RETYPED_TOL)
@@ -489,15 +489,15 @@ def long_cutoff(spec, cutoff, switch, want, nsteps=20, tol=1e-4):
 
 def test_water_at_cutoff_16():
     """tiled water, 64.6 A, cutoff 16 A: about 190 KB of staging by the initial estimate."""
-    kern = long_cutoff(water_spec(tiled_water(3)), 16.0, 14.0, (CLUSTER, FULL_ROWS))
+    kern = long_cutoff(water_spec(tiled_water(3)), 16.0, 14.0, (PAIR_CLUSTER, PAIR_ROWS_FX2))
     print("water x3^3 at cutoff 16: kernel", kern)
 
 
 def test_128_types_at_cutoff_14():
-    kern = long_cutoff(retyped(tiled_water(3), 128), 14.0, 12.0, (CLUSTER, FULL_ROWS), tol=RETYPED_TOL)
+    kern = long_cutoff(retyped(tiled_water(3), 128), 14.0, 12.0, (PAIR_CLUSTER, PAIR_ROWS_FX2), tol=RETYPED_TOL)
     print("128 types at cutoff 14: kernel", kern)
 
 
 def test_128_types_at_cutoff_12_stay_on_the_cluster_kernel():
     """About 167 KB of staging: within the limit, so the fall-back must not take it."""
-    long_cutoff(retyped(tiled_water(3), 128), 12.0, 10.0, (CLUSTER,), tol=RETYPED_TOL)
+    long_cutoff(retyped(tiled_water(3), 128), 12.0, 10.0, (PAIR_CLUSTER,), tol=RETYPED_TOL)

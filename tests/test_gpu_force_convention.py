@@ -32,6 +32,8 @@ import torch
 import test_gpu_cluster_systems as G
 from conftest import load_golden
 from oracle import refmd
+from torchmd_b200._lib import (PAIR_CLUSTER, PAIR_EWALD, PAIR_EWALD_CLUSTER, PAIR_EWALD_F64, PAIR_EWALD_FX, PAIR_EWALD_FX2,
+                               PAIR_F64, PAIR_OPEN_FX2, PAIR_ROWS, PAIR_ROWS_FX, PAIR_ROWS_FX2)
 
 pytestmark = [pytest.mark.gpu]
 DEV = "cuda:0"
@@ -80,23 +82,23 @@ def system_of(key):
 # (case id, system, environment, dtype, pme, kernel of an explicit call, kernel of an exact-gradient call)
 NOCL = {"TMD_B200_CLUSTER": "0"}
 MATRIX = [
-    ("k0_open", "ala2_nobox_rf", dict(NOCL, TMD_B200_FX="0"), F32, False, 0, 0),
-    ("k0_box_plain", "chain_plain", dict(NOCL, TMD_B200_FX="0"), F32, False, 0, 0),
-    ("k1", "chain_amber_periodic", dict(NOCL, TMD_B200_FX="1"), F32, False, 1, 1),
-    ("k2", "chain_amber_periodic", dict(NOCL, TMD_B200_FX="2"), F32, False, 2, 1),
-    ("k2_plain", "chain_plain", dict(NOCL, TMD_B200_FX="2"), F32, False, 2, 1),
-    ("k3", "ala2_nobox_rf", dict(NOCL, TMD_B200_FX="2"), F32, False, 3, 0),
-    ("k4_open", "ala2_nobox_rf", {"TMD_B200_CLUSTER": "1"}, F32, False, 4, 4),
-    ("k4_water", "water_x2", {"TMD_B200_CLUSTER": "1"}, F32, False, 4, 4),
-    ("k4_protein", "protein_x2", {"TMD_B200_CLUSTER": "1"}, F32, False, 4, 4),
-    ("k5", "chain_amber_periodic", {}, F64, False, 5, 5),
-    ("k5_plain", "chain_plain", {}, F64, False, 5, 5),
-    ("k6", "chain_amber_periodic", dict(NOCL, TMD_B200_FX="0"), F32, True, 6, 6),
-    ("k7", "chain_amber_periodic", dict(NOCL, TMD_B200_FX="1"), F32, True, 7, 7),
-    ("k8", "chain_amber_periodic", {}, F64, True, 8, 8),
-    ("k9", "chain_amber_periodic", dict(NOCL, TMD_B200_FX="2"), F32, True, 9, 7),
-    ("k10_water", "water_x2", {"TMD_B200_CLUSTER": "1"}, F32, True, 10, 10),
-    ("k10_protein", "protein_x2", {"TMD_B200_CLUSTER": "1"}, F32, True, 10, 10),
+    ("k0_open", "ala2_nobox_rf", dict(NOCL, TMD_B200_FX="0"), F32, False, PAIR_ROWS, PAIR_ROWS),
+    ("k0_box_plain", "chain_plain", dict(NOCL, TMD_B200_FX="0"), F32, False, PAIR_ROWS, PAIR_ROWS),
+    ("k1", "chain_amber_periodic", dict(NOCL, TMD_B200_FX="1"), F32, False, PAIR_ROWS_FX, PAIR_ROWS_FX),
+    ("k2", "chain_amber_periodic", dict(NOCL, TMD_B200_FX="2"), F32, False, PAIR_ROWS_FX2, PAIR_ROWS_FX),
+    ("k2_plain", "chain_plain", dict(NOCL, TMD_B200_FX="2"), F32, False, PAIR_ROWS_FX2, PAIR_ROWS_FX),
+    ("k3", "ala2_nobox_rf", dict(NOCL, TMD_B200_FX="2"), F32, False, PAIR_OPEN_FX2, PAIR_ROWS),
+    ("k4_open", "ala2_nobox_rf", {"TMD_B200_CLUSTER": "1"}, F32, False, PAIR_CLUSTER, PAIR_CLUSTER),
+    ("k4_water", "water_x2", {"TMD_B200_CLUSTER": "1"}, F32, False, PAIR_CLUSTER, PAIR_CLUSTER),
+    ("k4_protein", "protein_x2", {"TMD_B200_CLUSTER": "1"}, F32, False, PAIR_CLUSTER, PAIR_CLUSTER),
+    ("k5", "chain_amber_periodic", {}, F64, False, PAIR_F64, PAIR_F64),
+    ("k5_plain", "chain_plain", {}, F64, False, PAIR_F64, PAIR_F64),
+    ("k6", "chain_amber_periodic", dict(NOCL, TMD_B200_FX="0"), F32, True, PAIR_EWALD, PAIR_EWALD),
+    ("k7", "chain_amber_periodic", dict(NOCL, TMD_B200_FX="1"), F32, True, PAIR_EWALD_FX, PAIR_EWALD_FX),
+    ("k8", "chain_amber_periodic", {}, F64, True, PAIR_EWALD_F64, PAIR_EWALD_F64),
+    ("k9", "chain_amber_periodic", dict(NOCL, TMD_B200_FX="2"), F32, True, PAIR_EWALD_FX2, PAIR_EWALD_FX),
+    ("k10_water", "water_x2", {"TMD_B200_CLUSTER": "1"}, F32, True, PAIR_EWALD_CLUSTER, PAIR_EWALD_CLUSTER),
+    ("k10_protein", "protein_x2", {"TMD_B200_CLUSTER": "1"}, F32, True, PAIR_EWALD_CLUSTER, PAIR_EWALD_CLUSTER),
 ]
 CASES = {c[0]: c[1:] for c in MATRIX}
 
@@ -196,7 +198,7 @@ def big_water_orders(t=3, nsample=300):
         for exact in order:
             F = torch.zeros_like(pos)
             forces.compute(pos.detach().clone().requires_grad_(exact), box, F, explicit_forces=not exact)
-            assert _kernel(forces) == G.CLUSTER
+            assert _kernel(forces) == PAIR_CLUSTER
             err = np.abs(F[0].cpu().double().numpy()[atoms] - want[exact]).max()
             print(f"water x{t}^3, {order}, exact={exact}: {nsample} sampled atoms, max|dF| {err:.3e}")
             assert err < 1e-4, (order, exact, err)
@@ -234,7 +236,7 @@ def autograd_surfaces_after_explicit(spec, monkeypatch, nsteps=20, batch=2):
     def explicit_first(forces, p, b):
         F = torch.zeros_like(p)
         forces.compute(p, b, F)
-        assert _kernel(forces) == G.CLUSTER
+        assert _kernel(forces) == PAIR_CLUSTER
         assert np.abs(F.cpu().double().numpy() - np.concatenate([Fo_explicit] * p.shape[0])).max() < tol
 
     # backward
@@ -246,7 +248,7 @@ def autograd_surfaces_after_explicit(spec, monkeypatch, nsteps=20, batch=2):
     p = pos.detach().clone().requires_grad_(True)
     E = forces.compute(p, box, None, toNumpy=False, calculateForces=False, explicit_forces=False)
     E.sum().backward()
-    assert _kernel(forces) == G.CLUSTER
+    assert _kernel(forces) == PAIR_CLUSTER
     check(p.grad, "backward after explicit")
     e_tot = sum(Eo[0][k] for k in spec["terms"])
     assert abs(float(E.detach()[0]) - e_tot) <= 1e-5 * abs(e_tot) + 2e-3
@@ -258,7 +260,7 @@ def autograd_surfaces_after_explicit(spec, monkeypatch, nsteps=20, batch=2):
     Eb = torch.vmap(forces.compute, in_dims=(0,))(xb, box=box, forces=None, returnDetails=False, explicit_forces=False,
                                                   calculateForces=False, toNumpy=False)
     Eb.sum().backward()
-    assert _kernel(forces) == G.CLUSTER
+    assert _kernel(forces) == PAIR_CLUSTER
     for b in range(batch):
         check(xb.grad[b], f"vmap member {b}")
 
@@ -275,7 +277,7 @@ def autograd_surfaces_after_explicit(spec, monkeypatch, nsteps=20, batch=2):
 
     spy = Spy()
     minimize_pytorch_bfgs(system, spy, steps=1, max_iter=1)
-    assert len(spy.grads) == 1 and _kernel(forces) == G.CLUSTER
+    assert len(spy.grads) == 1 and _kernel(forces) == PAIR_CLUSTER
     check(spy.grads[0], "minimize_pytorch_bfgs evaluation")
 
     # MD after the autograd passes against MD on a context that never took one
@@ -290,7 +292,7 @@ def autograd_surfaces_after_explicit(spec, monkeypatch, nsteps=20, batch=2):
             check(p.grad, "backward before MD")
         integ = Integrator(system, forces, 1.0, DEV, gamma=None, T=None)
         _, pot, _ = integ.step(niter=nsteps)
-        assert _kernel(forces) == G.CLUSTER
+        assert _kernel(forces) == PAIR_CLUSTER
         out.append((system.pos.clone(), system.vel.clone(), pot))
     dp = (out[0][0] - out[1][0]).abs().max().item()
     dv = (out[0][1] - out[1][1]).abs().max().item()
@@ -458,7 +460,7 @@ def cluster_gradient_fp32(nsample=32, t=2):
     # the explicit convention on the same samples, for contrast: a bound that it met would not test the convention
     Fe = torch.zeros_like(pos)
     forces.compute(pos, boxes, Fe)
-    assert _kernel(forces) == G.CLUSTER
+    assert _kernel(forces) == PAIR_CLUSTER
     Fe = Fe[-1].cpu().double().numpy()
     fd = [-(E[2 * k] - E[2 * k + 1]) / (Xd[2 * k, a, ax] - Xd[2 * k + 1, a, ax]) for k, (a, ax) in enumerate(zip(atoms, axes))]
     far = max(abs(f - Fe[a, ax]) for f, a, ax in zip(fd, atoms, axes))

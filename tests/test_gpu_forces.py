@@ -22,6 +22,7 @@ import torch
 
 from conftest import golden_cfg, golden_system_tensors, load_golden, params_from_golden
 from oracle import refmd
+from torchmd_b200._lib import PAIR_CLUSTER
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -334,7 +335,7 @@ def test_nonperiodic_cutoff_with_distinct_replicas():
     f.compute(pos2, box, F2)
     assert (F2[1] - F[1]).abs().max().item() < 0.5
     from torchmd_b200 import _lib
-    if _lib.lib().tmd_pair_kernel(f._ctx) == 4:
+    if _lib.lib().tmd_pair_kernel(f._ctx) == PAIR_CLUSTER:
         # cluster half list: the partners' forces are summed by reductions at L2, in no fixed order
         tol = 5e-5 * max(1.0, F.abs().max().item() / 100.0)
         assert (F2[0] - F[0]).abs().max().item() < tol and (F2[2] - F[2]).abs().max().item() < tol

@@ -33,11 +33,11 @@ import torch
 
 from oracle import philox
 from oracle import refmd
+from torchmd_b200._lib import PAIR_CLUSTER
 
 pytestmark = [pytest.mark.gpu]
 DEV = "cuda:0"
 F32, F64 = torch.float32, torch.float64
-CLUSTER = 4  # tmd_pair_kernel id of the cluster half-list kernel (include/tmd_b200.h)
 POS_TOL32, VEL_TOL32 = 1e-4, 5e-4  # fp32 against fp64 after tens of steps (test_gpu_step_recovery, test_gpu_integrator)
 # fp32 water with its stiff O-H bonds (or the constraints of rigid water) on the cluster path, whose force sums have no
 # fixed order, against fp64: the bounds of test_gpu_cluster.test_gpu_cluster_md_follows_the_full_list_trajectory
@@ -154,23 +154,23 @@ def run_calls(integ, forces, calls):
 # (environment, calls, terms, stepwise, precision, kernel, launches per step of the last call)
 PATHS = {
     # k_vv_first_prepare -> (k_cpair + k_bonded) -> k_cstep_boundary x (n-1) ... -> k_cvv_second_fold
-    "cluster_fused_2": ({}, (2,), None, False, F32, CLUSTER, 4.5),
-    "cluster_fused_7": ({}, (7,), None, False, F32, CLUSTER, 29 / 7),
+    "cluster_fused_2": ({}, (2,), None, False, F32, PAIR_CLUSTER, 4.5),
+    "cluster_fused_7": ({}, (7,), None, False, F32, PAIR_CLUSTER, 29 / 7),
     # the same without the boundary kernel: k_cvv_second_fold every step
-    "cluster_fusestep0": ({"TMD_B200_FUSESTEP": "0"}, (7,), None, False, F32, CLUSTER, 5.0),
+    "cluster_fusestep0": ({"TMD_B200_FUSESTEP": "0"}, (7,), None, False, F32, PAIR_CLUSTER, 5.0),
     # bonded terms after the pair kernel on the same stream: k_bonded_vv_second
-    "cluster_overlap0": ({"TMD_B200_OVERLAP": "0"}, (7,), None, False, F32, CLUSTER, 3.0),
+    "cluster_overlap0": ({"TMD_B200_OVERLAP": "0"}, (7,), None, False, F32, PAIR_CLUSTER, 3.0),
     # the fused step issued kernel by kernel
-    "cluster_graph0": ({"TMD_B200_GRAPH": "0"}, (7,), None, False, F32, CLUSTER, 64 / 7),
+    "cluster_graph0": ({"TMD_B200_GRAPH": "0"}, (7,), None, False, F32, PAIR_CLUSTER, 64 / 7),
     # full Verlet rows with the overlapped bonded kernel: k_vv_second_fold
     "full_rows": ({"TMD_B200_CLUSTER": "0"}, (7,), None, False, F32, None, 5.0),
     # no bonded kinds: k_vv_second after the cluster pair kernel
-    "no_bonded": ({}, (7,), ["lj", "electrostatics"], False, F32, CLUSTER, 3.0),
+    "no_bonded": ({}, (7,), ["lj", "electrostatics"], False, F32, PAIR_CLUSTER, 3.0),
     # the duck-typed path: tmd_vv_first / compute / tmd_vv_second (k_vv_second)
-    "stepwise": ({}, (7,), None, True, F32, CLUSTER, 10.0),
+    "stepwise": ({}, (7,), None, True, F32, PAIR_CLUSTER, 10.0),
     # step(1) repeated and a split call on the default path
-    "single_steps": ({}, (1,) * 7, None, False, F32, CLUSTER, 5.0),
-    "split_3_4": ({}, (3, 4), None, False, F32, CLUSTER, 17 / 4),
+    "single_steps": ({}, (1,) * 7, None, False, F32, PAIR_CLUSTER, 5.0),
+    "split_3_4": ({}, (3, 4), None, False, F32, PAIR_CLUSTER, 17 / 4),
     # fp64: tmd_md_steps_f64 and the stepwise fp64 path (k_vv_second<double>)
     "fp64": ({}, (7,), None, False, F64, None, 12.0),
     "fp64_split": ({}, (3, 4), None, False, F64, None, 12.0),
@@ -191,7 +191,7 @@ def draw_case(monkeypatch, name, seed=SEED):
     if kernel is not None:
         assert kern == kernel, kern
     elif dtype == F32:
-        assert kern != CLUSTER, kern
+        assert kern != PAIR_CLUSTER, kern
     if per_step is not None:
         assert per == pytest.approx(per_step), per
     assert not st["overflow"] and st["force_calls"] == 1 + sum(calls), st
@@ -233,7 +233,7 @@ def test_step_word_carries_into_the_high_counter_word(dtype):
     st = forces.stats()
     assert not st["overflow"] and st["force_calls"] == 1 + n, st
     if dtype == F32:
-        assert _L().tmd_pair_kernel(forces._ctx) == CLUSTER
+        assert _L().tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER
     check_draws(system, integ, SEED, n, first_step=first, what=f"first_step 2^32-2 {dtype}")
 
 
@@ -332,7 +332,7 @@ def test_trajectory_fp32_cluster_water():
     dp, dv, forces = trajectory(F32, par, par64, sysd["coords"], sysd["box"], TERMS, CFG, 20, 1.0)
     shift = shift_scale(par64.masses, 1.0)
     print(f"fp32 cluster water 20 steps: dpos {dp:.2e} A, dvel {dv:.2e} A/tu (one-step noise shift {shift:.2f} A/tu)")
-    assert _L().tmd_pair_kernel(forces._ctx) == CLUSTER
+    assert _L().tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER
     assert 10 * WATER_VEL_TOL32 < shift
     assert dp < WATER_POS_TOL32 and dv < WATER_VEL_TOL32, (dp, dv)
 
@@ -379,7 +379,7 @@ def test_trajectory_fp32_rigid_water_cluster():
     par64 = testsystems.water_parameters(sysd, precision=F64)
     dp, dv, forces = trajectory(F32, par, par64, sysd["coords"], sysd["box"], TERMS, CFG, 20, 2.0, kind="water")
     print(f"fp32 rigid water, cluster path, 20 steps: dpos {dp:.2e} A, dvel {dv:.2e} A/tu")
-    assert _L().tmd_pair_kernel(forces._ctx) == CLUSTER
+    assert _L().tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER
     assert 10 * WATER_VEL_TOL32 < shift_scale(par64.masses, 2.0)
     assert dp < WATER_POS_TOL32 and dv < WATER_VEL_TOL32, (dp, dv)
 
@@ -455,7 +455,7 @@ def test_cluster_paths_agree_to_the_summation_order(monkeypatch):
         integ.seed = SEED
         for n in calls:
             integ.step(n)
-        assert _L().tmd_pair_kernel(forces._ctx) == CLUSTER
+        assert _L().tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER
         return system.pos.cpu().clone(), system.vel.cpu().clone()
 
     one = run((12,))

@@ -13,6 +13,7 @@ import os
 import numpy as np
 import pytest
 import torch
+from torchmd_b200._lib import PAIR_EWALD, PAIR_EWALD_CLUSTER, PAIR_EWALD_F64, PAIR_EWALD_FX, PAIR_EWALD_FX2
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -183,7 +184,7 @@ def _water_big(nw, dtype, nsample=None, seed=0, cutoff=9.0):
 
 def test_water10k_f64_against_the_oracle():
     kernel, grid, dF, fmax, dE = _water_big(3333, torch.float64)
-    assert kernel == 8 and grid == (45, 45, 45)
+    assert kernel == PAIR_EWALD_F64 and grid == (45, 45, 45)
     assert dF <= 1e-9 * fmax and dE <= 1e-9, (dF, fmax, dE)
 
 
@@ -228,27 +229,27 @@ def test_pme_kernels_only_with_pme(monkeypatch, nw_cluster=1200):
     7 k_pair_fx<MODE 2>, 8 k_ewpair64, 9 k_pair_fx2_ew, 10 k_cpair_ew -- and each one where its path applies."""
     from torchmd_b200 import _lib
 
-    ewald32 = (6, 7, 9, 10)
+    ewald32 = (PAIR_EWALD, PAIR_EWALD_FX, PAIR_EWALD_FX2, PAIR_EWALD_CLUSTER)
     for env in ({"TMD_B200_FX": "0"}, {"TMD_B200_FX": "1"}, {"TMD_B200_FX": "2"}, {"TMD_B200_CLUSTER": "1"}, {"TMD_B200_CLUSTER": "0"}):
         for k, v in env.items():
             monkeypatch.setenv(k, v)
-        for dtype, want in ((torch.float32, ewald32), (torch.float64, (8,))):
+        for dtype, want in ((torch.float32, ewald32), (torch.float64, (PAIR_EWALD_F64,))):
             sysd, par, _, terms, cfg = _water(200, dtype)  # (L = 18.2 A: the guard-free image holds at skin 0.5)
             for skin in (0.5, 3.0):  # 3 A: not the guard-free image (k_pair<SAFE = false>)
                 forces, *_ = _run(par, sysd["coords"][None], sysd["box"][None], terms, cfg, dtype, skin=skin)
                 got = _lib.lib().tmd_pair_kernel(forces._ctx)
                 assert got in want, (env, dtype, skin, got)
                 if dtype == torch.float32 and skin == 0.5:  # the guard-free image: the fixed-point kernels
-                    assert got == {"0": 6, "1": 7, "2": 9}.get(env.get("TMD_B200_FX"), got), (env, got)
+                    assert got == {"0": PAIR_EWALD, "1": PAIR_EWALD_FX, "2": PAIR_EWALD_FX2}.get(env.get("TMD_B200_FX"), got), (env, got)
                 if dtype == torch.float32 and skin == 3.0:
-                    assert got == 6, (env, got)
+                    assert got == PAIR_EWALD, (env, got)
         for k in env:
             monkeypatch.delenv(k)
     # a box the cluster lists take (L > 2 (rl + 8 A + skin)): the Ewald cluster kernel
     monkeypatch.setenv("TMD_B200_CLUSTER", "1")
     sysd, par, _, terms, cfg = _water(nw_cluster, torch.float32, jitter=0.7)
     forces, *_ = _run(par, sysd["coords"][None], sysd["box"][None], ["electrostatics"], dict(cutoff=6.0), torch.float32)
-    assert _lib.lib().tmd_pair_kernel(forces._ctx) == 10
+    assert _lib.lib().tmd_pair_kernel(forces._ctx) == PAIR_EWALD_CLUSTER
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float64])

@@ -20,11 +20,11 @@ import torch
 
 from oracle import philox
 from oracle import remd
+from torchmd_b200._lib import PAIR_CLUSTER
 
 pytestmark = [pytest.mark.gpu]
 DEV = "cuda:0"
 F32, F64 = torch.float32, torch.float64
-CLUSTER = 4  # tmd_pair_kernel id of the cluster half-list kernel
 SEED = 0x2545F4914F6CDD1D & (2**62 - 1)
 TIE = 1e-12  # a decision may differ from the oracle's only where |u - exp(D)| is below this
 
@@ -137,7 +137,7 @@ def test_equal_temperatures_are_the_scalar_run(monkeypatch, dtype):
     integ, _ = run(b, fb, [300.0] * 3, (50,))
     assert integ.vcoeff.shape == (3, a.natoms, 1)
     if dtype == F32:
-        assert _L().tmd_pair_kernel(fb._ctx) != CLUSTER
+        assert _L().tmd_pair_kernel(fb._ctx) != PAIR_CLUSTER
     assert torch.equal(a.pos, b.pos) and torch.equal(a.vel, b.vel)
 
 
@@ -166,7 +166,7 @@ def test_equal_temperatures_on_the_cluster_path():
         system, forces, _ = water_system(F32, 2, cluster=True)
         l0 = forces.stats()["kernel_launches"]
         run(system, forces, T, (12,))
-        assert _L().tmd_pair_kernel(forces._ctx) == CLUSTER
+        assert _L().tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER
         assert (forces.stats()["kernel_launches"] - l0) / 12 == pytest.approx(4.0 + 1 / 12)  # the fused step
         out.append((system.pos.cpu(), system.vel.cpu()))
     dp, dv = (out[0][0] - out[1][0]).abs().max().item(), (out[0][1] - out[1][1]).abs().max().item()
@@ -223,7 +223,7 @@ def decision_case(monkeypatch, name):
     if name == "cluster":
         temps = temps[:4]
         system, forces, _ = water_system(F32, 4, cluster=True)
-        kernel = CLUSTER
+        kernel = PAIR_CLUSTER
     elif name in ("full_rows", "fp64"):
         from test_gpu_step_recovery import full_rows
 
@@ -317,7 +317,7 @@ def test_exchanges_keep_the_captured_steps(monkeypatch):
     l0 = forces.stats()["kernel_launches"]
     integ.step(7)
     assert (forces.stats()["kernel_launches"] - l0) / 7 == pytest.approx(29 / 7)  # k_cstep_boundary between the steps
-    assert _L().tmd_pair_kernel(forces._ctx) == CLUSTER and _L().tmd_step_captures(forces._ctx) == c0
+    assert _L().tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER and _L().tmd_step_captures(forces._ctx) == c0
     xi = philox.langevin_noise(SEED, 7, 2, n, np.float32, position=position)
     vc = integ.vcoeff.cpu().numpy()[:, :, 0]
     got = system.vel.cpu().numpy().astype(np.float64)

@@ -32,11 +32,11 @@ import pytest
 import torch
 
 from oracle import refmd
+from torchmd_b200._lib import PAIR_CLUSTER, PAIR_EWALD_CLUSTER, PAIR_EWALD_F64, PAIR_EWALD_FX2
 
 pytestmark = [pytest.mark.gpu]
 DEV = "cuda:0"
 F32, F64 = torch.float32, torch.float64
-CLUSTER, EW64, EW_ROWS, EW_CLUSTER = 4, 8, 9, 10  # tmd_pair_kernel ids (include/tmd_b200.h)
 SEED = 0x5DEECE66D
 LANGEVIN = (1.0, 300.0)  # gamma in 1/ps, T in K
 ORACLE_MAX_ATOMS = 3000
@@ -279,40 +279,40 @@ def one_step_short(case_fn, dtype, calls, integ_kw):
 # (environment, system, precision, calls, stepwise, injected noise, pair kernel, launches per step of the last call)
 PATHS = {
     # k_vv_first_prepare -> (k_cpair + k_bonded) -> k_cstep_boundary ... -> k_cvv_second_fold; variants 2, 3 and 4
-    "cluster_fused_2": ({}, "water8k", F32, (2, 2, 2), False, False, CLUSTER, 4.5),
-    "cluster_fused_7": ({}, "water8k", F32, (7, 7, 7), False, False, CLUSTER, 29 / 7),
+    "cluster_fused_2": ({}, "water8k", F32, (2, 2, 2), False, False, PAIR_CLUSTER, 4.5),
+    "cluster_fused_7": ({}, "water8k", F32, (7, 7, 7), False, False, PAIR_CLUSTER, 29 / 7),
     # k_cvv_second_fold every step: variants 0 and 1
-    "cluster_fusestep0": ({"TMD_B200_FUSESTEP": "0"}, "water8k", F32, (7, 7, 7), False, False, CLUSTER, 5.0),
+    "cluster_fusestep0": ({"TMD_B200_FUSESTEP": "0"}, "water8k", F32, (7, 7, 7), False, False, PAIR_CLUSTER, 5.0),
     # the bonded energies from k_bonded_vv_second on the same stream
-    "cluster_overlap0": ({"TMD_B200_OVERLAP": "0"}, "water8k", F32, (7, 7, 7), False, False, CLUSTER, 3.0),
+    "cluster_overlap0": ({"TMD_B200_OVERLAP": "0"}, "water8k", F32, (7, 7, 7), False, False, PAIR_CLUSTER, 3.0),
     # the fused step issued kernel by kernel: the energy memset outside a graph
-    "cluster_graph0": ({"TMD_B200_GRAPH": "0"}, "water8k", F32, (7, 7, 7), False, False, CLUSTER, 64 / 7),
+    "cluster_graph0": ({"TMD_B200_GRAPH": "0"}, "water8k", F32, (7, 7, 7), False, False, PAIR_CLUSTER, 64 / 7),
     # full Verlet rows, overlapped bonded kernel, k_vv_second_fold
     "full_rows": ({"TMD_B200_CLUSTER": "0"}, "water8k", F32, (7, 7, 7), False, False, None, 5.0),
     "full_rows_graph0": ({"TMD_B200_CLUSTER": "0", "TMD_B200_GRAPH": "0"}, "water8k", F32, (5, 5, 5), False, False, None, None),
     # the duck-typed path: pot from the last compute, ke from k_vv_second
-    "stepwise": ({}, "water8k", F32, (3, 3, 3), True, False, CLUSTER, None),
-    "single_steps": ({}, "water8k", F32, (1, 1, 1), False, False, CLUSTER, None),
-    "split_3_4": ({}, "water8k", F32, (3, 4, 3), False, False, CLUSTER, None),
+    "stepwise": ({}, "water8k", F32, (3, 3, 3), True, False, PAIR_CLUSTER, None),
+    "single_steps": ({}, "water8k", F32, (1, 1, 1), False, False, PAIR_CLUSTER, None),
+    "split_3_4": ({}, "water8k", F32, (3, 4, 3), False, False, PAIR_CLUSTER, None),
     # injected noise: no graph, no fused step
-    "noise": ({}, "water8k", F32, (3, 3, 3), False, True, CLUSTER, None),
+    "noise": ({}, "water8k", F32, (3, 3, 3), False, True, PAIR_CLUSTER, None),
     # tmd_md_steps_f64 and the stepwise fp64 path
     "fp64": ({}, "water8k", F64, (5, 5, 5), False, False, None, None),
     "fp64_split": ({}, "water8k", F64, (2, 3, 1), False, False, None, None),
     "fp64_stepwise": ({}, "water8k", F64, (3, 3, 3), True, False, None, None),
     # the PME energy chain: cluster Ewald kernel, full rows, fp64
-    "pme_cluster": ({}, "water8k_pme", F32, (5, 5, 5), False, False, EW_CLUSTER, None),
-    "pme_full_rows": ({"TMD_B200_CLUSTER": "0"}, "water8k_pme", F32, (5, 5, 5), False, False, EW_ROWS, None),
-    "pme_fp64": ({}, "water8k_pme", F64, (3, 3, 3), False, False, EW64, None),
+    "pme_cluster": ({}, "water8k_pme", F32, (5, 5, 5), False, False, PAIR_EWALD_CLUSTER, None),
+    "pme_full_rows": ({"TMD_B200_CLUSTER": "0"}, "water8k_pme", F32, (5, 5, 5), False, False, PAIR_EWALD_FX2, None),
+    "pme_fp64": ({}, "water8k_pme", F64, (3, 3, 3), False, False, PAIR_EWALD_F64, None),
     # ke from the velocity constraint: rigid water (cluster path in fp32), X-H bonds of ala2
-    "rigid_water": ({}, "water8k_rigid", F32, (5, 5, 5), False, False, CLUSTER, None),
+    "rigid_water": ({}, "water8k_rigid", F32, (5, 5, 5), False, False, PAIR_CLUSTER, None),
     "rigid_water_fp64": ({}, "water8k_rigid", F64, (3, 3, 3), False, False, None, None),
     "hbonds": ({}, "ala2_hbonds", F32, (5, 5, 5), False, False, None, None),
     "hbonds_fp64": ({}, "ala2_hbonds", F64, (5, 5, 5), False, False, None, None),
     # CMAP under dihedrals, 1-4 under lj / electrostatics, from the overlapped bonded kernel
     "cmap": ({}, "ala2_cmap", F32, (5, 5, 5), False, False, None, None),
     "cmap_fp64": ({}, "ala2_cmap", F64, (5, 5, 5), False, False, None, None),
-    "pairs14_cluster": ({}, "protein", F32, (7, 7, 7), False, False, CLUSTER, None),
+    "pairs14_cluster": ({}, "protein", F32, (7, 7, 7), False, False, PAIR_CLUSTER, None),
 }
 
 
@@ -331,7 +331,7 @@ def energy_case(monkeypatch, name):
     if kernel is not None:
         assert kern == kernel, (name, kern)
     elif dtype == F32:
-        assert kern not in (CLUSTER, EW_CLUSTER), (name, kern)
+        assert kern not in (PAIR_CLUSTER, PAIR_EWALD_CLUSTER), (name, kern)
     if per_step is not None and not rebuilt:
         assert per == pytest.approx(per_step), (name, per)
     assert not st["overflow"], st
@@ -497,7 +497,7 @@ def test_md_steps_host_matches_md_steps(monkeypatch):
                 state = (s.pos.cpu().clone(), s.vel.cpu().clone())
             assert not f.stats()["overflow"]
             res.append((n, state, ene.copy(), ke.copy()))
-        assert _L().tmd_pair_kernel(f._ctx) not in (CLUSTER, EW_CLUSTER)
+        assert _L().tmd_pair_kernel(f._ctx) not in (PAIR_CLUSTER, PAIR_EWALD_CLUSTER)
     dev, hst = res[:2], res[2:]
     for (n, (p0, v0), e0, k0), (_, (p1, v1), e1, k1) in zip(dev, hst):
         assert torch.equal(p0, p1) and torch.equal(v0, v1), n

@@ -14,6 +14,7 @@ import pytest
 import torch
 
 import test_simt_kernels as T
+from torchmd_b200._lib import PAIR_ROWS_FX2
 
 
 class _Stream:
@@ -352,7 +353,7 @@ def test_round2_default_configuration_passes_the_gpu_tests(hostsim_r2, capsys):
     from conftest import load_golden
 
     f, *_ = G.run_gpu(load_golden("chain_amber_periodic"))
-    assert hostsim_r2.tmd_pair_kernel(f._ctx) == 2  # the packed fixed-point kernel is what ran
+    assert hostsim_r2.tmd_pair_kernel(f._ctx) == PAIR_ROWS_FX2  # the packed fixed-point kernel is what ran
     G.test_api_errors_and_formats()
     I.test_nve_trajectory_matches_reference()
     I.test_langevin_with_injected_noise_matches_reference()

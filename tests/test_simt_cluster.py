@@ -11,6 +11,7 @@ import torch
 import test_simt_kernels as T
 from conftest import load_golden
 from oracle import refmd
+from torchmd_b200._lib import PAIR_CLUSTER, PAIR_ROWS
 
 
 @pytest.fixture(scope="module")
@@ -90,7 +91,7 @@ def test_cluster_path_periodic_water(host_cl, thrown):
         sh = rng.integers(-thrown, thrown + 1, size=coords.shape).astype(np.float32)
         coords = coords + sh * (rng.random(len(coords)) < 0.3)[:, None] * np.float32(L)
     system, forces, e = _compute(sysd, coords, host_cl)
-    assert host_cl.tmd_pair_kernel(forces._ctx) == 4, "the cluster kernel did not run"
+    assert host_cl.tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER, "the cluster kernel did not run"
     f64, e_ref, pairs_ref = _oracle(sysd, system)
     pairs = forces.neighbour_pairs(system.pos, system.box).numpy()
     assert pairs.shape == pairs_ref.shape and np.array_equal(pairs, pairs_ref.astype(np.int32))
@@ -116,7 +117,7 @@ def test_cluster_exact_pass_decides_band_pairs(host_cl):
         shift = (coords[a].astype(np.float64) + u * float(r)) - coords[b].astype(np.float64)
         coords[b : b + 3] = (coords[b : b + 3].astype(np.float64) + shift).astype(np.float32)
     system, forces, e = _compute(sysd, coords, host_cl)
-    assert host_cl.tmd_pair_kernel(forces._ctx) == 4
+    assert host_cl.tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER
     f64, e_ref, pairs_ref = _oracle(sysd, system)
     pairs = forces.neighbour_pairs(system.pos, system.box).numpy()
     assert np.array_equal(pairs, pairs_ref.astype(np.int32))
@@ -132,7 +133,7 @@ def test_cluster_path_without_a_box(simt_cl, name):
     g = load_golden(name)
     c = T.Ctx(simt_cl, g)
     F, E = c.forces()
-    assert simt_cl.tmd_pair_kernel(c.h) == 4
+    assert simt_cl.tmd_pair_kernel(c.h) == PAIR_CLUSTER
     T.check_against_golden(c, F, E)
     F2, _ = c.forces(energies=False)
     T.check_against_golden(c, F2, {})
@@ -150,13 +151,13 @@ def test_cluster_list_capacity_grows_and_lattice_falls_back(host_cl, monkeypatch
     coords = np.array(sysd["coords"], dtype=np.float32)
     monkeypatch.setenv("TMD_B200_CLUSTER_ECAP", "64")  # start far too small
     system, forces, e = _compute(sysd, coords, host_cl)
-    assert host_cl.tmd_pair_kernel(forces._ctx) == 4
+    assert host_cl.tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER
     f64, e_ref, _ = _oracle(sysd, system)
     assert (system.forces.double() - f64).abs().max().item() < 1e-4
     monkeypatch.delenv("TMD_B200_CLUSTER_ECAP")
     lat = testsystems.water_box(1500, seed=0)  # lattice start, 35.5 A box: some cell rows hold only a few atoms
     system, forces, e = _compute(lat, np.array(lat["coords"], dtype=np.float32), host_cl)
-    assert host_cl.tmd_pair_kernel(forces._ctx) == 0, "expected the fall-back to the full rows"
+    assert host_cl.tmd_pair_kernel(forces._ctx) == PAIR_ROWS, "expected the fall-back to the full rows"
     f64, e_ref, pairs_ref = _oracle(lat, system)
     assert (system.forces.double() - f64).abs().max().item() < 1e-4 * max(1.0, f64.abs().max().item() / 100.0)
     assert np.array_equal(forces.neighbour_pairs(system.pos, system.box).numpy(), pairs_ref.astype(np.int32))
@@ -181,7 +182,7 @@ def test_cluster_md_steps_follow_the_full_list_trajectory(host_cl, monkeypatch):
         integ = Integrator(system, forces, 1.0, "cpu", gamma=None, T=None)
         ekin, pot, temp = integ.step(niter=12)
         st = forces.stats()
-        assert host_cl.tmd_pair_kernel(forces._ctx) == (4 if cluster == "1" else 0)
+        assert host_cl.tmd_pair_kernel(forces._ctx) == (PAIR_CLUSTER if cluster == "1" else PAIR_ROWS)
         assert st["rebuilds"] >= 2, st
         out.append((system.pos.clone(), system.vel.clone(), ekin, pot))
     # (stiff O-H bonds, 900 kcal/mol/A^2, turn a 4e-6 A difference in position into 3e-3 in force and 7e-5 in velocity)
@@ -216,7 +217,7 @@ def test_step_boundary_kernel_reproduces_the_two_kernel_sequence(host_cl, monkey
             ekin, pot, temp = integ.step(niter=niter)
             res.append((float(ekin[0]), float(pot[0])))
         st = forces.stats()
-        assert host_cl.tmd_pair_kernel(forces._ctx) == 4 and st["rebuilds"] >= 2, st
+        assert host_cl.tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER and st["rebuilds"] >= 2, st
         out.append((system.pos.clone(), system.vel.clone(), system.forces.clone(), res, st["kernel_launches"]))
     if os.environ.get("SIMT_SCHEDULE"):
         # another thread order: the partner forces are summed by reductions in whatever order the warps run, so even two
@@ -249,7 +250,7 @@ def test_cluster_path_with_owned_atom_ranges(host_cl):
     sysd = tiled_water(2)
     coords = np.array(sysd["coords"], dtype=np.float32)
     system, forces, e_full = _compute(sysd, coords, host_cl)
-    assert host_cl.tmd_pair_kernel(forces._ctx) == 4
+    assert host_cl.tmd_pair_kernel(forces._ctx) == PAIR_CLUSTER
     F_full = system.forces.clone()
     n = len(coords)
     world = 3
@@ -266,7 +267,7 @@ def test_cluster_path_with_owned_atom_ranges(host_cl):
         f2._ensure_box(s2.box)
         _lib.check(host_cl.tmd_set_owned_atoms(ctx, lo, hi - lo))
         e = f2.compute(s2.pos, s2.box, s2.forces, returnDetails=True)[0]
-        assert host_cl.tmd_pair_kernel(ctx) == 4
+        assert host_cl.tmd_pair_kernel(ctx) == PAIR_CLUSTER
         assert (s2.forces[0, lo:hi] - F_full[0, lo:hi]).abs().max().item() < 3e-5
         for k in TERMS:
             e_sum[k] += e[k]

@@ -10,6 +10,7 @@ import pytest
 
 import test_simt_kernels as T
 from conftest import load_golden
+from torchmd_b200._lib import PAIR_CLUSTER
 
 
 @pytest.fixture(scope="module")
@@ -61,7 +62,7 @@ def test_standalone_calls_after_md_steps_are_those_of_a_fresh_context(simt_cl, m
     monkeypatch.setenv("TMD_B200_GRAPH", graph)
     ran, fresh = setup(simt_cl), setup(simt_cl)
     T.md_steps(simt_cl, ran, 3)
-    assert simt_cl.tmd_pair_kernel(ran.h) == 4
+    assert simt_cl.tmd_pair_kernel(ran.h) == PAIR_CLUSTER
     pos, vel, F0 = ran.posw.copy(), ran.vel.copy(), ran.F.copy()
     got = standalone_calls(simt_cl, ran, pos, vel.copy(), F0)
     want = standalone_calls(simt_cl, fresh, pos, vel.copy(), F0)

@@ -28,6 +28,24 @@ ENERGY_SLOTS = (
 NUM_ENERGIES = len(ENERGY_SLOTS)
 
 
+# tmd_pair_kernel() ids (include/tmd_b200.h): the non-bonded pair kernel the last force call ran
+PAIR_ROWS, PAIR_ROWS_FX, PAIR_ROWS_FX2, PAIR_OPEN_FX2, PAIR_CLUSTER, PAIR_F64 = 0, 1, 2, 3, 4, 5
+PAIR_EWALD, PAIR_EWALD_FX, PAIR_EWALD_F64, PAIR_EWALD_FX2, PAIR_EWALD_CLUSTER = 6, 7, 8, 9, 10
+PAIR_KERNEL_NAMES = {
+    PAIR_ROWS: "k_pair (full rows)",
+    PAIR_ROWS_FX: "k_pair_fx (full rows, fixed point)",
+    PAIR_ROWS_FX2: "k_pair_fx2 (full rows, fixed point, fp32x2)",
+    PAIR_OPEN_FX2: "k_pair2_open (full rows without a box, fp32x2)",
+    PAIR_CLUSTER: "k_cpair (cluster half list)",
+    PAIR_F64: "k_pair_f64 (full rows, fp64)",
+    PAIR_EWALD: "k_pair (full rows, real-space Ewald)",
+    PAIR_EWALD_FX: "k_pair_fx (full rows, fixed point, real-space Ewald)",
+    PAIR_EWALD_F64: "k_ewpair64 (full rows, fp64, real-space Ewald)",
+    PAIR_EWALD_FX2: "k_pair_fx2_ew (full rows, fixed point, fp32x2, real-space Ewald)",
+    PAIR_EWALD_CLUSTER: "k_cpair_ew (cluster half list, real-space Ewald)",
+}
+
+
 def term_mask(terms):
     m = 0
     for t in terms:

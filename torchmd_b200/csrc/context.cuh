@@ -189,11 +189,8 @@ struct tmd_ctx {
   bool have_atoms = false, have_nonbonded = false, have_box = false, have_excl = false;
   bool excl_is_set = true;           // the exclusion CSR lists every pair in both rows, once, and no atom with itself
   bool periodic = false;
-  bool safe_image = false;           // guard-free minimum image valid (see min_image_fast)
-  int pair_mode = 0;                 // 1: LJ+switch + reaction-field Coulomb specialisation
   int exact_gradient = 0;            // tmd_set_force_convention: switched-LJ force as the true gradient
-  int last_pair_kernel = 0;          // tmd_pair_kernel(): 0 float (k_pair), 1 k_pair_fx, 2 k_pair_fx2, 3 k_pair2_open
-  bool fx_packed = false;            // TMD_B200_FX=2: k_pair_fx2 (fp32x2 arithmetic) where it applies
+  int last_pair_kernel = 0;          // tmd_pair_kernel(): the PairKernel of the last force call (tmd_b200.cu, enqueue_pair)
   int4* xf_buf = nullptr;            // fixed-point records (periodic pair kernel), owned; d.xf_s points here when in use
   bool cluster_failed = false;       // the cluster path reported F_CLFAIL: full rows until cluster_retry_at force calls
   int64_t cluster_retry_at = 0, cluster_retry_after = 0;

@@ -110,11 +110,12 @@ inline void launch_smem(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t 
 // f(a, b) with a and b as std::integral_constant<bool, ...>: one launch line for the four <bool, bool> instantiations
 // of a kernel, as in with_bools(thermo, ke != nullptr, [&](auto th, auto e) { launch(k_vv_second<float, th, e>, ...); })
 template <typename F>
+inline void with_bool(bool a, F&& f) {
+  a ? f(std::true_type{}) : f(std::false_type{});
+}
+template <typename F>
 inline void with_bools(bool a, bool b, F&& f) {
-  using T = std::true_type;
-  using N = std::false_type;
-  if (a) b ? f(T{}, T{}) : f(T{}, N{});
-  else b ? f(N{}, T{}) : f(N{}, N{});
+  with_bool(a, [&](auto x) { with_bool(b, [&](auto y) { f(x, y); }); });
 }
 
 struct DeviceGuard {
@@ -181,7 +182,18 @@ struct StepArgs {
   const int* ladder;  // temperature index of each replica (tmd_set_temperature_ladder), or null: part of the step-graph key
 };
 
+// The pair path finalize chose for the box and the system (plan_pairs); pair_kernel_of picks each call's kernel from it.
+struct PairPlan {
+  bool cluster = false;     // cluster half lists (cluster.cuh)
+  bool safe_image = false;  // guard-free minimum image (min_image_fast): no listed pair can be 0.45 L apart
+  bool rows_fx = false;     // full rows on fixed-point records (k_pair_fx; TMD_B200_FX=1 or 2)
+  bool packed = false;      // TMD_B200_FX=2: fp32x2 arithmetic where a kernel has it
+  bool grid_fx = false;     // the cell grids carry fixed-point units: rows_fx, or the cluster path in a box
+  double cl_max_extent = INFINITY;  // cluster path in a box: the longest cluster the smallest box takes (A)
+};
+
 struct CtxPriv {
+  PairPlan pair;
   // TMD_B200_OVERLAP=1: bonded kernel on a second stream, concurrent with the pair kernel
   cudaStream_t side = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -244,7 +256,6 @@ struct CtxPriv {
   int64_t step_captures = 0;        // tmd_step_captures: captures of a tmd_md_steps step graph
   // tmd_rescale_box: the cell grids of the boxes held (host copy), the choices finalize made that a rescale must keep
   std::vector<Grid> grids;
-  bool grid_fx = false;             // the grids carry fixed-point units (k_pair_fx, cluster path)
   bool rescaled = false;            // cl.max_extent has been set to the bound every fast-path box keeps
   double cl_bound = 0.0;            // that bound (A)
   double* box_dev = nullptr;        // (R,3) box lengths on the device, for tmd_scale_molecules
@@ -279,11 +290,6 @@ static int need_precision(tmd_ctx* ctx, int bits, const char* name) {
 
 // ---- particle-mesh Ewald: parameter choice (the one place it is made) ------------------------
 static inline bool pme_on(tmd_ctx* ctx) { return priv(ctx).pme_tol > 0.0; }
-// MODE of the full-row pair kernels (physics.cuh, pair_terms): a PME context never runs another
-static int pair_mode_of(tmd_ctx* ctx) {
-  if (pme_on(ctx)) return 2;
-  return (ctx->pair_mask == (T_LJ | T_ELEC) && ctx->d.pp.has_switch && ctx->d.pp.rfa && !ctx->exact_gradient) ? 1 : 0;
-}
 static int smallest_235(int n) {
   for (int m = std::max(n, 1);; ++m) {
     int k = m;
@@ -1036,8 +1042,22 @@ static int pme_finalize(tmd_ctx* ctx, cudaStream_t stream) {
   return TMD_OK;
 }
 
+// ---- box conditions of the pair paths: finalize chooses with them, tmd_rescale_box keeps them ----------------------
+static float box_min(const std::vector<float>& L) { return *std::min_element(L.begin(), L.end()); }
+// no listed pair is further apart than this (A); margin: list_margin
+static double pair_reach(const tmd_ctx* ctx, double margin) { return ctx->cutoff + 2.0 * ctx->skin + 2.0 * margin; }
+// the guard-free minimum image (min_image_fast) is valid iff no listed pair can be 0.45 L apart
+static bool guard_free_image(const tmd_ctx* ctx, double margin, double lmin) { return pair_reach(ctx, margin) < 0.45 * lmin; }
+// the longest cluster a box of smallest length lmin takes: a pair of a list, |x_i - x_j| <= rl + extent + skin along
+// every axis, must stay below half a box length (the fixed-point separations wrap to the minimum image by themselves)
+static double cluster_extent_limit(const tmd_ctx* ctx, double rl, double lmin) { return 0.5 * lmin - rl - ctx->skin - 0.05; }
+// fp64 contexts build the list from an fp32 shadow of the positions, which holds box lengths up to 4096 A
+static bool f64_box_fits(const std::vector<float>& L) {
+  return std::none_of(L.begin(), L.end(), [](float x) { return x > 4096.f; });
+}
+
 // Cell grid of one replica's box L (list radius rl, ctx->d.nsub cells per radius), and the fixed-point units of the
-// pair kernels when priv(ctx).grid_fx.  keep: the cell counts the replica's grid had, which a rescale keeps while the
+// pair kernels when PairPlan::grid_fx.  keep: the cell counts the replica's grid had, which a rescale keeps while the
 // cells stay at least rl / nsub wide (a growing box only widens them) and otherwise lowers to floor(L nsub / rl) --
 // never above the counts the cell arrays were sized for.  null: chosen from the box.  Returns false when a kept grid
 // would fall below 2 nsub + 1 cells along an axis.
@@ -1073,14 +1093,13 @@ static bool box_grid(tmd_ctx* ctx, Grid& g, const float* L3, double rl, double m
     g.ncells *= g.n[k];
     lmax = std::max(lmax, (double)L);
   }
-  if (priv(ctx).grid_fx) {
+  if (priv(ctx).pair.grid_fx) {
     for (int k = 0; k < 3; ++k) {
       g.fx_unit[k] = (float)((double)g.L[k] / 4294967296.0);
       g.fx_inv[k] = 4294967296.0 / (double)g.L[k];
     }
-    const double rmax = ctx->cutoff + 2.0 * ctx->skin + 2.0 * margin;  // no listed pair is further apart
     double c0, c1;
-    fx_margin(rmax, lmax, &c0, &c1);
+    fx_margin(pair_reach(ctx, margin), lmax, &c0, &c1);
     g.fx_c0 = (float)(c0 * 1.0000002);  // never round the bound down
     g.fx_c1 = (float)(c1 * 1.0000002);
   }
@@ -1111,6 +1130,62 @@ static ClSizing cluster_sizing(const tmd_ctx* ctx, double rl, int nsub, double m
   s.mcap = std::max(64, keep_mcap);
   s.smem = (size_t)CL_WARPS * 2 * ((size_t)(s.mcap + s.ecap) * sizeof(unsigned) + s.mcap) + (size_t)CL_WARPS * ctx->d.ntypes * CL_H * sizeof(ClTab);
   return s;
+}
+
+// pair terms out of {lj, electrostatics}: the cluster kernels and the fp32x2 full-row kernels evaluate no others
+static bool lj_el_terms(const tmd_ctx* ctx) { return ctx->pair_mask != 0 && (ctx->pair_mask & ~(T_LJ | T_ELEC)) == 0; }
+
+// The pair path of the context's box and system, the one decision of finalize that pair_kernel_of reads; reads
+// TMD_B200_CLUSTER and TMD_B200_FX.  *cl_size: the cluster lists' capacities and staging when the plan takes them.
+static PairPlan plan_pairs(tmd_ctx* ctx, double rl, double margin, double max_density, int cl_nsub, ClSizing* cl_size) {
+  const bool has_cut = ctx->cutoff >= 0, f64 = ctx->precision == 64;
+  const double lmin = box_min(ctx->box_host);
+  PairPlan p;
+  // Cluster half-list path (cluster.cuh): a cutoff, pair terms out of {lj, electrostatics}, few atom types, the
+  // whole system on this context; in a periodic box additionally every pair a list can hold must have ONE image within
+  // reach (cluster_extent_limit).  Otherwise: full Verlet rows.  Either force convention: the launch picks the
+  // kernel, so the path never depends on which convention the first call asked for.
+  const double cl_extent = 8.0;  // a periodic box must leave room for clusters at least this long (A)
+  p.cluster = env_switch("TMD_B200_CLUSTER", TMD_DEFAULT_CLUSTER) == 1 && !f64 && !ctx->cluster_failed && has_cut &&
+              lj_el_terms(ctx) && ctx->d.ntypes <= CL_MAXT && ctx->natoms < (1 << 24) - 4096 * CL;
+  if (p.cluster && ctx->periodic) {
+    p.cl_max_extent = cluster_extent_limit(ctx, rl, lmin);
+    p.cluster = p.cl_max_extent >= cl_extent;
+  }
+  if (p.cluster) {
+    // the lists must fit k_cpair's shared-memory staging (long cutoffs, many atom types): otherwise the full rows.  When
+    // only the capacities grown after an overflow do not fit, the context gives up the cluster lists as after F_CLFAIL
+    // and tries them again later with fresh capacities.
+    const ClSizing fresh = cluster_sizing(ctx, rl, cl_nsub, max_density, 0, 0);
+    *cl_size = cluster_sizing(ctx, rl, cl_nsub, max_density, ctx->d.cl.ecap, ctx->d.cl.mcap);
+    if (fresh.smem > CL_SMEM_MAX) {
+      p.cluster = false;
+    } else if (cl_size->smem > CL_SMEM_MAX) {
+      p.cluster = false;
+      ctx->cluster_failed = true;
+      ctx->cluster_retry_after = std::min<int64_t>(std::max<int64_t>(2 * ctx->cluster_retry_after, 1000), 1 << 20);
+      ctx->cluster_retry_at = ctx->force_calls + ctx->cluster_retry_after;
+    }
+  }
+  p.safe_image = ctx->periodic && has_cut && guard_free_image(ctx, margin, lmin);
+  // Fixed-point separations on the full rows (k_pair_fx): a periodic box with the guard-free image (TMD_B200_FX=1 or 2)
+  const int fx = env_switch("TMD_B200_FX", TMD_DEFAULT_FX);
+  p.packed = fx == 2;
+  p.rows_fx = (fx == 1 || fx == 2) && p.safe_image && ctx->pair_mask && !f64 && !p.cluster;
+  p.grid_fx = p.rows_fx || (p.cluster && ctx->periodic);
+  return p;
+}
+
+// The cluster pair kernel of (E, box, PME, exact-gradient convention): what enqueue_pair launches, and the list finalize
+// gives the dynamic shared memory to.
+using ClusterKernel = void (*)(DeviceState, SwitchConsts, double*);
+static ClusterKernel cluster_kernel(bool e, bool periodic, bool ewald, bool grad) {
+  ClusterKernel k = nullptr;
+  with_bools(e, periodic, [&](auto E, auto P) {
+    if (ewald) k = grad ? k_cpair_ew_grad<E> : k_cpair_ew<E>;
+    else k = grad ? k_cpair_grad<E, P> : k_cpair<E, P>;
+  });
+  return k;
 }
 
 static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
@@ -1154,73 +1229,25 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   // With the fp32 slack of the build arithmetic and binning (0.004 A) the radius needs 26h + 7h = 33h more; 36h =
   // 0.0088 A is added.
   const double margin = list_margin(ctx);  // A
-  if (f64 && ctx->periodic)
-    for (int e = 0; e < R * 3; ++e)
-      if (ctx->box_host[e] > 4096.f)
-        return fail(TMD_ERR_UNSUPPORTED, "fp64 contexts take box lengths up to 4096 A (the fp32 shadow of the list build)");
+  if (f64 && ctx->periodic && !f64_box_fits(ctx->box_host))
+    return fail(TMD_ERR_UNSUPPORTED, "fp64 contexts take box lengths up to 4096 A (the fp32 shadow of the list build)");
   const double rl = has_cut ? ctx->cutoff + ctx->skin + margin : INFINITY;
   d.rlist = (float)rl;
   d.rlist2 = has_cut ? (float)(rl * rl) : INFINITY;
   d.trigger2 = has_cut ? (float)(0.25 * ctx->skin * ctx->skin) : INFINITY;
 
-  // Cluster half-list path (cluster.cuh): a cutoff, pair terms out of {lj, electrostatics}, few atom types, the
-  // whole system on this context; in a periodic box additionally every pair a list can hold must have ONE image within
-  // reach (size condition below).  Otherwise: full Verlet rows.  Either force convention: the launch picks the
-  // kernel, so the path never depends on which convention the first call asked for.
   ClusterState& cl = d.cl;
-  const double cl_extent = 8.0;  // a periodic box must leave room for clusters at least this long (A)
-  bool use_cluster = env_switch("TMD_B200_CLUSTER", TMD_DEFAULT_CLUSTER) == 1 && !f64 && !ctx->cluster_failed && has_cut &&
-                     ctx->pair_mask != 0 && (ctx->pair_mask & ~(T_LJ | T_ELEC)) == 0 &&
-                     d.ntypes <= CL_MAXT && N < (1 << 24) - 4096 * CL;
-  double cl_max_extent = INFINITY;
-  if (use_cluster && ctx->periodic) {
-    // pair (i, j) of a list: |x_i - x_j| <= rl + (cluster extent) + skin along every axis, and that must stay below
-    // half a box length (cluster.cuh)
-    float lmin = INFINITY;
-    for (int e = 0; e < R * 3; ++e) lmin = std::min(lmin, ctx->box_host[e]);
-    // (the fixed-point separations wrap to the minimum image by themselves: a listed pair only has to stay below
-    //  half a box length, rl + extent + skin < L / 2)
-    cl_max_extent = 0.5 * (double)lmin - rl - ctx->skin - 0.05;
-    use_cluster = cl_max_extent >= cl_extent;
-  }
   double max_density = 0.0;  // atoms per A^3 of the densest replica box
   if (ctx->periodic)
     for (int r = 0; r < R; ++r)
       max_density = std::max(max_density, N / ((double)ctx->box_host[r * 3] * ctx->box_host[r * 3 + 1] * ctx->box_host[r * 3 + 2]));
   const int cl_nsub = std::max(1, (int)floor(rl / 4.0 + 0.5));  // cluster path: cells of about 4 A
   ClSizing cl_size{};
-  if (use_cluster) {
-    // the lists must fit k_cpair's shared-memory staging (long cutoffs, many atom types): otherwise the full rows.  When
-    // only the capacities grown after an overflow do not fit, the context gives up the cluster lists as after F_CLFAIL
-    // and tries them again later with fresh capacities.
-    const ClSizing fresh = cluster_sizing(ctx, rl, cl_nsub, max_density, 0, 0);
-    cl_size = cluster_sizing(ctx, rl, cl_nsub, max_density, cl.ecap, cl.mcap);
-    if (fresh.smem > CL_SMEM_MAX) {
-      use_cluster = false;
-    } else if (cl_size.smem > CL_SMEM_MAX) {
-      use_cluster = false;
-      ctx->cluster_failed = true;
-      ctx->cluster_retry_after = std::min<int64_t>(std::max<int64_t>(2 * ctx->cluster_retry_after, 1000), 1 << 20);
-      ctx->cluster_retry_at = ctx->force_calls + ctx->cluster_retry_after;
-    }
-  }
+  const PairPlan plan = priv(ctx).pair = plan_pairs(ctx, rl, margin, max_density, cl_nsub, &cl_size);
+  const bool use_cluster = plan.cluster;
   d.nsub = use_cluster ? cl_nsub : 2;
-
-  // guard-free minimum image is valid iff no listed pair can be further than 0.45 L apart
-  ctx->safe_image = false;
-  if (ctx->periodic && has_cut) {
-    float lmin = INFINITY;
-    for (int e = 0; e < R * 3; ++e) lmin = std::min(lmin, ctx->box_host[e]);
-    ctx->safe_image = (ctx->cutoff + 2.0 * ctx->skin + 2.0 * margin) < 0.45 * (double)lmin;
-  }
-  d.check_far = ctx->safe_image ? 1 : 0;
+  d.check_far = plan.safe_image ? 1 : 0;
   d.pp.true_gradient = ctx->exact_gradient;
-  ctx->pair_mode = pair_mode_of(ctx);
-  // Fixed-point separations in the pair kernel (k_pair_fx): periodic box with the guard-free
-  // image condition (TMD_B200_FX=1 or 2).
-  const int fx = env_switch("TMD_B200_FX", TMD_DEFAULT_FX);
-  ctx->fx_packed = fx == 2;
-  priv(ctx).grid_fx = (((fx == 1 || fx == 2) && ctx->safe_image) || (use_cluster && ctx->periodic)) && ctx->pair_mask && !f64;
 
   // cell grid per replica
   std::vector<Grid> grids(R);
@@ -1236,7 +1263,7 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   d.build_split = (ctx->periodic && max_cells < ctx->nsm) ? (int)std::min<long long>(64, (ctx->nsm + max_cells - 1) / max_cells) : 1;
 
   d.xf_s = nullptr;
-  if (priv(ctx).grid_fx && !use_cluster) {
+  if (plan.rows_fx) {
     const size_t n = (size_t)R * N + R;
     if ((rc = device_alloc(&ctx->xf_buf, n))) return rc;
     TMD_CUDA(cudaMemset(ctx->xf_buf, 0, n * sizeof(int4)));
@@ -1283,7 +1310,7 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
       cl.max_rows = (int)rows;
       cl.slots = (int)slots;
       cl.nclusters_cap = (int)(slots / CL);
-      cl.max_extent = (float)cl_max_extent;
+      cl.max_extent = (float)plan.cl_max_extent;
       cl.ecap = cl_size.ecap;
       cl.mcap = cl_size.mcap;
       auto grab = [&](auto** ptr, size_t n) {
@@ -1320,13 +1347,9 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
       pv.cl_smem = cl_size.smem;  // (at most CL_SMEM_MAX: decided above)
 #if !defined(TMD_SIMT_HOST)
       int per_sm = 0;
-      const void* kernels[12] = {(const void*)k_cpair<false, false>, (const void*)k_cpair<false, true>,
-                                 (const void*)k_cpair<true, false>, (const void*)k_cpair<true, true>,
-                                 (const void*)k_cpair_ew<false>, (const void*)k_cpair_ew<true>,
-                                 (const void*)k_cpair_grad<false, false>, (const void*)k_cpair_grad<false, true>,
-                                 (const void*)k_cpair_grad<true, false>, (const void*)k_cpair_grad<true, true>,
-                                 (const void*)k_cpair_ew_grad<false>, (const void*)k_cpair_ew_grad<true>};
-      for (const void* k : kernels) TMD_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pv.cl_smem));
+      for (int b = 0; b < 16; ++b)  // every (E, box, PME, convention) of cluster_kernel
+        TMD_CUDA(cudaFuncSetAttribute((const void*)cluster_kernel(b & 1, b & 2, b & 4, b & 8),
+                                      cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pv.cl_smem));
       TMD_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cpair<false, true>, CL_WARPS * 32, pv.cl_smem));
       pv.cl_blocks = std::max(1, std::min(ctx->nsm * std::max(per_sm, 1), (cl.nclusters_cap + CL_WARPS - 1) / CL_WARPS));
 #else
@@ -1458,95 +1481,100 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
   return TMD_OK;
 }
 
-// Particle-mesh Ewald (a periodic box) on the full rows: the real-space Ewald instantiations of the same kernels the
-// context would run without it, and nothing else.  tmd_pair_kernel(): 6 k_pair<MODE 2>, 7 k_pair_fx<MODE 2>,
-// 9 k_pair_fx2_ew (the cluster path: 10 k_cpair_ew).
-static void launch_pair_ewald(tmd_ctx* ctx, dim3 pg, cudaStream_t st, float* forces, double* energies) {
-  const bool e = energies != nullptr, small = ctx->d.ntypes <= FX_SMALLT_MAX;
+// ---- the pair kernel of a force call: one choice (pair_kernel_of), one launch (enqueue_pair) ----------------------
+// tmd_pair_kernel() ids, in the order of include/tmd_b200.h (torchmd_b200/_lib.py names them the same); enqueue_pair
+// shows the kernel of each
+enum PairKernel : int {
+  PAIR_ROWS, PAIR_ROWS_FX, PAIR_ROWS_FX2, PAIR_OPEN_FX2, PAIR_CLUSTER, PAIR_F64,
+  PAIR_EWALD, PAIR_EWALD_FX, PAIR_EWALD_F64, PAIR_EWALD_FX2, PAIR_EWALD_CLUSTER
+};
+struct PairChoice {
+  PairKernel kernel;
+  int mode;         // MODE of k_pair / k_pair_fx (physics.cuh, pair_terms): 2 PME, 1 switched LJ + reaction field, 0 any
+  bool small;       // SMALLT: the LJ table of the fixed-point and fp32x2 kernels is staged in shared memory
+  bool safe_image;  // SAFE: the guard-free minimum image
+};
+// From the plan of the last finalisation and what may change between calls without one: the force convention.  Particle-
+// mesh Ewald runs the real-space Ewald instantiations of the kernels the context would run without it.  The fp32x2
+// kernels have no exact-gradient instantiation, and they evaluate lj and electrostatics only.
+static PairChoice pair_kernel_of(tmd_ctx* ctx) {
+  const PairPlan& p = priv(ctx).pair;
+  const bool pme = pme_on(ctx), grad = ctx->exact_gradient != 0;
+  const bool packed = p.packed && lj_el_terms(ctx) && !grad;
+  PairChoice c;
+  c.mode = pme ? 2 : (ctx->pair_mask == (T_LJ | T_ELEC) && ctx->d.pp.has_switch && ctx->d.pp.rfa && !grad) ? 1 : 0;
+  c.small = ctx->d.ntypes <= FX_SMALLT_MAX;
+  c.safe_image = p.safe_image;
+  if (ctx->precision == 64) c.kernel = pme ? PAIR_EWALD_F64 : PAIR_F64;
+  else if (p.cluster) c.kernel = pme ? PAIR_EWALD_CLUSTER : PAIR_CLUSTER;
+  else if (pme) c.kernel = !p.rows_fx ? PAIR_EWALD : packed ? PAIR_EWALD_FX2 : PAIR_EWALD_FX;
+  else if (p.rows_fx) c.kernel = packed ? PAIR_ROWS_FX2 : PAIR_ROWS_FX;
+  else c.kernel = (!ctx->periodic && packed) ? PAIR_OPEN_FX2 : PAIR_ROWS;
+  return c;
+}
+
+// Launches the pair kernel k on grid (the caller's: its owned rows in fp32, all rows in fp64, the persistent CTAs of
+// the cluster kernels), between the pair-kernel timing events (tmd_profile_begin).  forces: in the context's precision.
+static int enqueue_pair(tmd_ctx* ctx, PairChoice k, dim3 grid, void* forces, double* energies, cudaStream_t st) {
+  CtxPriv& pv = priv(ctx);
+  const DeviceState& d = ctx->d;
+  float* f = static_cast<float*>(forces);
+  double* f64 = static_cast<double*>(forces);
+  const bool e = energies != nullptr, grad = ctx->exact_gradient != 0;
   const int th = PAIR_WARPS * 32;
-  const bool lj_el_only = ctx->pair_mask != 0 && (ctx->pair_mask & ~(T_LJ | T_ELEC)) == 0;
-  if (ctx->d.xf_s && ctx->fx_packed && lj_el_only && !ctx->exact_gradient && ctx->d.ntypes <= 128) {
-    ctx->last_pair_kernel = 9;
-    const SwitchConsts sc = make_switch_consts_ewald(ctx->d.pp);
-    if (e && small) launch(k_pair_fx2_ew<true, true>, pg, th, st, ctx->d, sc, forces, energies);
-    else if (e) launch(k_pair_fx2_ew<true, false>, pg, th, st, ctx->d, sc, forces, energies);
-    else if (small) launch(k_pair_fx2_ew<false, true>, pg, th, st, ctx->d, sc, forces, energies);
-    else launch(k_pair_fx2_ew<false, false>, pg, th, st, ctx->d, sc, forces, energies);
-    return;
+  const bool sample = pv.profiling && (size_t)(pv.ev_used + 2) <= pv.ev.size();
+  if (sample) TMD_CUDA(cudaEventRecord(pv.ev[pv.ev_used], st));
+  ctx->last_pair_kernel = k.kernel;
+  switch (k.kernel) {
+    case PAIR_ROWS:  // (SAFE only in a box)
+      with_bools(e, k.mode == 1, [&](auto E, auto M) {
+        constexpr int mode = decltype(M)::value;
+        if (!ctx->periodic) launch(k_pair<E, false, false, mode>, grid, th, st, d, f, energies);
+        else if (k.safe_image) launch(k_pair<E, true, true, mode>, grid, th, st, d, f, energies);
+        else launch(k_pair<E, true, false, mode>, grid, th, st, d, f, energies);
+      });
+      break;
+    case PAIR_ROWS_FX:
+      with_bools(e, k.small, [&](auto E, auto S) {
+        if (k.mode == 1) launch(k_pair_fx<E, 1, S>, grid, th, st, d, f, energies);
+        else launch(k_pair_fx<E, 0, S>, grid, th, st, d, f, energies);
+      });
+      break;
+    case PAIR_ROWS_FX2:
+      with_bools(e, k.small, [&](auto E, auto S) { launch(k_pair_fx2<E, S>, grid, th, st, d, make_switch_consts(d.pp), f, energies); });
+      break;
+    case PAIR_OPEN_FX2:
+      with_bools(e, k.small, [&](auto E, auto S) { launch(k_pair2_open<E, S>, grid, th, st, d, make_switch_consts(d.pp), f, energies); });
+      break;
+    case PAIR_EWALD:
+      with_bools(e, k.safe_image, [&](auto E, auto S) { launch(k_pair<E, true, S, 2>, grid, th, st, d, f, energies); });
+      break;
+    case PAIR_EWALD_FX:
+      with_bools(e, k.small, [&](auto E, auto S) { launch(k_pair_fx<E, 2, S>, grid, th, st, d, f, energies); });
+      break;
+    case PAIR_EWALD_FX2:
+      with_bools(e, k.small, [&](auto E, auto S) { launch(k_pair_fx2_ew<E, S>, grid, th, st, d, make_switch_consts_ewald(d.pp), f, energies); });
+      break;
+    case PAIR_CLUSTER:
+      launch_smem(cluster_kernel(e, ctx->periodic, false, grad), grid, CL_WARPS * 32, pv.cl_smem, st, d, make_switch_consts(d.pp), energies);
+      break;
+    case PAIR_EWALD_CLUSTER:
+      launch_smem(cluster_kernel(e, true, true, grad), grid, CL_WARPS * 32, pv.cl_smem, st, d, make_switch_consts_ewald(d.pp), energies);
+      break;
+    case PAIR_F64:
+      with_bools(e, ctx->periodic, [&](auto E, auto P) { launch(k_pair_f64<E, P>, grid, th, st, d, ctx->d64, f64, energies); });
+      break;
+    case PAIR_EWALD_F64:
+      with_bool(e, [&](auto E) { launch(k_ewpair64<E>, grid, th, st, d, ctx->d64, f64, energies); });
+      break;
   }
-  if (ctx->d.xf_s) {
-    ctx->last_pair_kernel = 7;
-    if (e && small) launch(k_pair_fx<true, 2, true>, pg, th, st, ctx->d, forces, energies);
-    else if (e) launch(k_pair_fx<true, 2, false>, pg, th, st, ctx->d, forces, energies);
-    else if (small) launch(k_pair_fx<false, 2, true>, pg, th, st, ctx->d, forces, energies);
-    else launch(k_pair_fx<false, 2, false>, pg, th, st, ctx->d, forces, energies);
-    return;
+  const char* name = (k.kernel == PAIR_F64 || k.kernel == PAIR_EWALD_F64) ? "k_pair_f64" : "k_pair";
+  TMD_LAUNCHED(ctx, name);
+  if (sample) {
+    TMD_CUDA(cudaEventRecord(pv.ev[pv.ev_used + 1], st));
+    pv.ev_used += 2;
   }
-  ctx->last_pair_kernel = 6;
-  if (ctx->safe_image) {
-    if (e) launch(k_pair<true, true, true, 2>, pg, th, st, ctx->d, forces, energies);
-    else launch(k_pair<false, true, true, 2>, pg, th, st, ctx->d, forces, energies);
-  } else {
-    if (e) launch(k_pair<true, true, false, 2>, pg, th, st, ctx->d, forces, energies);
-    else launch(k_pair<false, true, false, 2>, pg, th, st, ctx->d, forces, energies);
-  }
-}
-template <bool E, bool P, bool SAFE>
-static void launch_pair_mode(tmd_ctx* ctx, dim3 pg, cudaStream_t st, float* forces, double* energies) {
-  if (ctx->pair_mode == 1) launch(k_pair<E, P, SAFE, 1>, pg, PAIR_WARPS * 32, st, ctx->d, forces, energies);
-  else launch(k_pair<E, P, SAFE, 0>, pg, PAIR_WARPS * 32, st, ctx->d, forces, energies);
-}
-template <bool E>
-static void launch_pair_fx(tmd_ctx* ctx, dim3 pg, cudaStream_t st, float* forces, double* energies) {
-  const bool small = ctx->d.ntypes <= FX_SMALLT_MAX;
-  const int th = PAIR_WARPS * 32;
-  // TMD_B200_FX=2: fp32x2 arithmetic for the term sets made of "lj" and "electrostatics"
-  const bool lj_el_only = ctx->pair_mask != 0 && (ctx->pair_mask & ~(T_LJ | T_ELEC)) == 0;
-  if (ctx->fx_packed && lj_el_only && !ctx->exact_gradient && ctx->d.ntypes <= 128) {
-    ctx->last_pair_kernel = 2;
-    const SwitchConsts sc = make_switch_consts(ctx->d.pp);
-    if (small) launch(k_pair_fx2<E, true>, pg, th, st, ctx->d, sc, forces, energies);
-    else launch(k_pair_fx2<E, false>, pg, th, st, ctx->d, sc, forces, energies);
-    return;
-  }
-  ctx->last_pair_kernel = 1;
-  if (ctx->pair_mode == 1) {
-    if (small) launch(k_pair_fx<E, 1, true>, pg, th, st, ctx->d, forces, energies);
-    else launch(k_pair_fx<E, 1, false>, pg, th, st, ctx->d, forces, energies);
-  } else {
-    if (small) launch(k_pair_fx<E, 0, true>, pg, th, st, ctx->d, forces, energies);
-    else launch(k_pair_fx<E, 0, false>, pg, th, st, ctx->d, forces, energies);
-  }
-}
-static void launch_pair(tmd_ctx* ctx, dim3 pg, cudaStream_t st, float* forces, double* energies) {
-  const bool e = energies != nullptr;
-  ctx->last_pair_kernel = 0;
-  if (pme_on(ctx)) {
-    launch_pair_ewald(ctx, pg, st, forces, energies);
-  } else if (ctx->d.xf_s) {
-    if (e) launch_pair_fx<true>(ctx, pg, st, forces, energies);
-    else launch_pair_fx<false>(ctx, pg, st, forces, energies);
-  } else if (!ctx->periodic && ctx->fx_packed && ctx->pair_mask != 0 && (ctx->pair_mask & ~(T_LJ | T_ELEC)) == 0 &&
-             !ctx->exact_gradient) {
-    // TMD_B200_FX=2 without a box: fp32x2 arithmetic on the float records
-    ctx->last_pair_kernel = 3;
-    const SwitchConsts sc = make_switch_consts(ctx->d.pp);
-    const bool small = ctx->d.ntypes <= FX_SMALLT_MAX;
-    const int th = PAIR_WARPS * 32;
-    if (e && small) launch(k_pair2_open<true, true>, pg, th, st, ctx->d, sc, forces, energies);
-    else if (e) launch(k_pair2_open<true, false>, pg, th, st, ctx->d, sc, forces, energies);
-    else if (small) launch(k_pair2_open<false, true>, pg, th, st, ctx->d, sc, forces, energies);
-    else launch(k_pair2_open<false, false>, pg, th, st, ctx->d, sc, forces, energies);
-  } else if (!ctx->periodic) {
-    if (e) launch_pair_mode<true, false, false>(ctx, pg, st, forces, energies);
-    else launch_pair_mode<false, false, false>(ctx, pg, st, forces, energies);
-  } else if (ctx->safe_image) {
-    if (e) launch_pair_mode<true, true, true>(ctx, pg, st, forces, energies);
-    else launch_pair_mode<false, true, true>(ctx, pg, st, forces, energies);
-  } else {
-    if (e) launch_pair_mode<true, true, false>(ctx, pg, st, forces, energies);
-    else launch_pair_mode<false, true, false>(ctx, pg, st, forces, energies);
-  }
+  return TMD_OK;
 }
 
 static inline dim3 atoms_grid(const tmd_ctx* ctx, int threads) {
@@ -1671,23 +1699,7 @@ static int enqueue_forces_f64(tmd_ctx* ctx, const double* pos, double* forces, d
     const bool pme = pme_on(ctx);
     if (pme)
       if (int rc = enqueue_pme_chain<double>(ctx, pos, energies, st)) return rc;
-    CtxPriv& pv = priv(ctx);
-    const bool sample = pv.profiling && (size_t)(pv.ev_used + 2) <= pv.ev.size();
-    if (sample) TMD_CUDA(cudaEventRecord(pv.ev[pv.ev_used], st));
-    const dim3 pg((N + PAIR_WARPS - 1) / PAIR_WARPS, R);
-    const int th = PAIR_WARPS * 32;
-    ctx->last_pair_kernel = pme ? 8 : 5;
-    if (pme && energies) launch(k_ewpair64<true>, pg, th, st, d, D, forces, energies);
-    else if (pme) launch(k_ewpair64<false>, pg, th, st, d, D, forces, energies);
-    else if (energies && ctx->periodic) launch(k_pair_f64<true, true>, pg, th, st, d, D, forces, energies);
-    else if (energies) launch(k_pair_f64<true, false>, pg, th, st, d, D, forces, energies);
-    else if (ctx->periodic) launch(k_pair_f64<false, true>, pg, th, st, d, D, forces, energies);
-    else launch(k_pair_f64<false, false>, pg, th, st, d, D, forces, energies);
-    TMD_LAUNCHED(ctx, "k_pair_f64");
-    if (sample) {
-      TMD_CUDA(cudaEventRecord(pv.ev[pv.ev_used + 1], st));
-      pv.ev_used += 2;
-    }
+    if (int rc = enqueue_pair(ctx, pair_kernel_of(ctx), dim3((N + PAIR_WARPS - 1) / PAIR_WARPS, R), forces, energies, st)) return rc;
     if (pme)
       if (int rc = enqueue_pme_gather<double>(ctx, pos, forces, energies, st)) return rc;
   } else {
@@ -1847,46 +1859,9 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
       TMD_CUDA(cudaStreamUpdateCaptureDependencies(st, &cond_node, 1, cudaStreamSetCaptureDependencies));
     }
 
-    const dim3 pg((std::max(d.own_n, 1) + PAIR_WARPS - 1) / PAIR_WARPS, R);
     CtxPriv& pv = priv(ctx);
-    const bool sample = pv.profiling && (size_t)(pv.ev_used + 2) <= pv.ev.size();
-    if (sample) TMD_CUDA(cudaEventRecord(pv.ev[pv.ev_used], st));
-    // (the cluster kernels: the explicit convention, or the exact-gradient instantiations of the same kernels)
-    const bool grad = ctx->exact_gradient != 0;
-    if (d.cl.on && pme) {
-      ctx->last_pair_kernel = 10;
-      const SwitchConsts sc = make_switch_consts_ewald(d.pp);
-      const dim3 cg(pv.cl_blocks, R);
-      if (grad && energies) launch_smem(k_cpair_ew_grad<true>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
-      else if (grad) launch_smem(k_cpair_ew_grad<false>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
-      else if (energies) launch_smem(k_cpair_ew<true>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
-      else launch_smem(k_cpair_ew<false>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
-    } else if (d.cl.on && grad) {
-      ctx->last_pair_kernel = 4;
-      const SwitchConsts sc = make_switch_consts(d.pp);
-      const dim3 cg(pv.cl_blocks, R);
-      const bool e = energies != nullptr;
-      if (e && ctx->periodic) launch_smem(k_cpair_grad<true, true>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
-      else if (e) launch_smem(k_cpair_grad<true, false>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
-      else if (ctx->periodic) launch_smem(k_cpair_grad<false, true>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
-      else launch_smem(k_cpair_grad<false, false>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
-    } else if (d.cl.on) {
-      ctx->last_pair_kernel = 4;
-      const SwitchConsts sc = make_switch_consts(d.pp);
-      const dim3 cg(pv.cl_blocks, R);
-      const bool e = energies != nullptr;
-      if (e && ctx->periodic) launch_smem(k_cpair<true, true>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
-      else if (e) launch_smem(k_cpair<true, false>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
-      else if (ctx->periodic) launch_smem(k_cpair<false, true>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
-      else launch_smem(k_cpair<false, false>, cg, CL_WARPS * 32, pv.cl_smem, st, d, sc, energies);
-    } else {
-      launch_pair(ctx, pg, st, forces, energies);
-    }
-    TMD_LAUNCHED(ctx, "k_pair");
-    if (sample) {
-      TMD_CUDA(cudaEventRecord(pv.ev[pv.ev_used + 1], st));
-      pv.ev_used += 2;
-    }
+    const dim3 pg = d.cl.on ? dim3(pv.cl_blocks, R) : dim3((std::max(d.own_n, 1) + PAIR_WARPS - 1) / PAIR_WARPS, R);
+    if (int rc = enqueue_pair(ctx, pair_kernel_of(ctx), pg, forces, energies, st)) return rc;
     if (pme) {
       TMD_CUDA(cudaStreamWaitEvent(st, pv.pme_join, 0));
       if (int prc = enqueue_pme_gather<float>(ctx, pos, forces, energies, st)) return prc;
@@ -2384,7 +2359,6 @@ int tmd_set_force_convention(tmd_ctx* ctx, int exact_gradient) {
   ctx->exact_gradient = exact_gradient ? 1 : 0;
   ctx->d.pp.true_gradient = ctx->exact_gradient;  // uniform kernel parameter: takes effect at the next launch
   ctx->d64.pp.true_gradient = ctx->exact_gradient;
-  ctx->pair_mode = pair_mode_of(ctx);
   return TMD_OK;
 }
 
@@ -2511,24 +2485,21 @@ static int rescale_box(tmd_ctx* ctx, const T* box_diag, tmd_stream stream, const
   const bool f64 = ctx->precision == 64;
   std::vector<float> b32(box_diag, box_diag + R * 3);
   std::vector<double> b64(box_diag, box_diag + R * 3);
-  float lmin = INFINITY;
-  for (int e = 0; e < R * 3; ++e) lmin = std::min(lmin, b32[e]);
-  if (f64)
-    for (int e = 0; e < R * 3; ++e)
-      if (b32[e] > 4096.f) return fail(TMD_ERR_UNSUPPORTED, who + "fp64 contexts take box lengths up to 4096 A");
+  const double lmin = box_min(b32);
+  if (f64 && !f64_box_fits(b32)) return fail(TMD_ERR_UNSUPPORTED, who + "fp64 contexts take box lengths up to 4096 A");
   const double margin = list_margin(ctx), rl = ctx->cutoff + ctx->skin + margin;
-  if (ctx->safe_image && !((ctx->cutoff + 2.0 * ctx->skin + 2.0 * margin) < 0.45 * (double)lmin))
+  if (pv.pair.safe_image && !guard_free_image(ctx, margin, lmin))
     return fail(TMD_ERR_UNSUPPORTED, who + "the box is too small for the guard-free minimum image the context was set up with");
   double cl_bound = pv.cl_bound;
   if (ctx->d.cl.on) {
     // cl.max_extent is held by value in the captured steps: at the first rescale it becomes the bound of a box 10 %
     // shorter than the one finalised (at least the 8 A the path needs), and every later box must keep it
-    const double limit = 0.5 * (double)lmin - rl - ctx->skin - 0.05;
+    const double limit = cluster_extent_limit(ctx, rl, lmin);
     if (!pv.rescaled) {
       float lmin0 = INFINITY;
       for (const Grid& g : pv.grids)
         for (int k = 0; k < 3; ++k) lmin0 = std::min(lmin0, g.L[k]);
-      cl_bound = std::max(8.0, std::min((double)ctx->d.cl.max_extent, 0.5 * 0.9 * (double)lmin0 - rl - ctx->skin - 0.05));
+      cl_bound = std::max(8.0, std::min((double)ctx->d.cl.max_extent, cluster_extent_limit(ctx, rl, 0.9 * (double)lmin0)));
     }
     if (limit < cl_bound) return fail(TMD_ERR_UNSUPPORTED, who + "the box is too small for the cluster lists' extent bound");
   }

@@ -431,7 +431,7 @@ def bench_decomposed(args, world, rank, local, config):
         },
         "gpu_launches": int(launches.item()),
         "roofline": {
-            "kernel": "non-bonded pair kernel (id %d: 4 = cluster half list, 2 = fixed-point full rows), slowest rank; timed over %d eager steps after the graph-replayed timed region" % (int(L.tmd_pair_kernel(forces._ctx)), nprof),
+            "kernel": "non-bonded pair kernel %s, slowest rank; timed over %d eager steps after the graph-replayed timed region" % (_lib.PAIR_KERNEL_NAMES[int(L.tmd_pair_kernel(forces._ctx))], nprof),
             "bound": "hbm",
             "achieved": (32.0 * n / world + 4.0 * int(count.item()) / world) / (pair_avg_ms * 1e-3) / 1e9 if pair_avg_ms > 0 else 0.0,
             "peak": peak,
