@@ -406,6 +406,27 @@ int tmd_replica_exchange(tmd_ctx* ctx, const double* energies_dev, int stride, i
 int tmd_replica_exchange_f64(tmd_ctx* ctx, const double* energies_dev, int stride, int nterms, uint64_t seed,
                              uint64_t attempt, double* vel_dev, int64_t* counts_dev, tmd_stream stream);
 
+/* ---- Generalized Born implicit solvent, OBC2 (library version >= 108) ----
+ *
+ * tmd_set_gb(ctx, n = natoms, radius, screen, solvent_dielectric, surface_tension) turns on OBC2
+ * (AMBER igb=5) for a system without a box; n = 0 turns it off.  radius (A, above 0.09) and screen
+ * (positive) are fp64 host arrays for either precision, e.g. a prmtop's RADII and SCREEN.  Per atom
+ * rho = R - 0.09, S = screen rho; I_i = sum over j != i of the HCT descreening term of sphere j
+ * (csrc/gbsa.cuh); psi = rho I / 2; B = 1 / (1/rho - tanh(psi - 0.8 psi^2 + 4.85 psi^3) / R).  The
+ * electrostatic energy slot then also holds
+ *   polar      -1/2 k (1 - 1/eps) sum_i sum_j qi qj / f_ij,  f_ij = sqrt(r^2 + Bi Bj exp(-r^2 / 4 Bi Bj)),
+ *              over every i and j (i = j included, no exclusions), k the Coulomb constant of tmd_set_nonbonded
+ *   non-polar  sum_i 4 pi sigma (R_i + 1.4)^2 (R_i / B_i)^6, sigma = surface_tension (kcal/mol/A^2; 0: none)
+ * and the forces are its exact gradient, the chain through every Born radius included.  The solute
+ * dielectric is 1.  Each pass gives every atom its own warp and sums in fp64 in a fixed order, so the
+ * GB forces are bitwise reproducible.  TMD_ERR_ARG for n other than 0 or natoms, a radius <= 0.09 A,
+ * a screen <= 0, a non-finite value, a dielectric <= 0 or a negative surface tension;
+ * TMD_ERR_UNSUPPORTED (here when already known, otherwise at the first force call) for a periodic box,
+ * a cutoff, the reaction field, particle-mesh Ewald, no electrostatics term, and a decomposed context.
+ * tmd_set_owned_atoms and tmd_dd_* return TMD_ERR_UNSUPPORTED on a GB context. */
+int tmd_set_gb(tmd_ctx* ctx, int n, const double* radius_host, const double* screen_host, double solvent_dielectric,
+               double surface_tension);
+
 /* ---- inspection ------------------------------------------------------------ */
 
 /* The reference's neighbour list for one replica: every non-excluded pair

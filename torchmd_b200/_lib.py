@@ -143,6 +143,8 @@ _SIGNATURES = {
     "tmd_set_temperature_ladder": (C.c_int, [_P, C.c_int, _P, _P]),
     "tmd_replica_exchange": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_uint64, C.c_uint64, _P, _P, _P]),
     "tmd_replica_exchange_f64": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_uint64, C.c_uint64, _P, _P, _P]),
+    # OBC2 implicit solvent (library version >= 108)
+    "tmd_set_gb": (C.c_int, [_P, C.c_int, _P, _P, C.c_double, C.c_double]),
 }
 ERR_UNSUPPORTED = -5
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
@@ -161,8 +163,8 @@ def lib():
                 "torchmd_b200 has no CPU or PyTorch fallback."
             )
         handle = C.CDLL(LIB_PATH)
-        if not hasattr(handle, "tmd_set_temperature_ladder"):
-            raise ImportError(f"{LIB_PATH} predates the replica-exchange entry points: rebuild it (__graft_entry__.build())")
+        if not hasattr(handle, "tmd_set_gb"):
+            raise ImportError(f"{LIB_PATH} predates the implicit-solvent entry point: rebuild it (__graft_entry__.build())")
         for name, (res, args) in _SIGNATURES.items():
             fn = getattr(handle, name)
             fn.restype = res

@@ -29,6 +29,8 @@ semantics step by step:
   1-based atom indices, ``CHARMM_UREY_BRADLEY_FORCE_CONSTANT`` (kcal/mol/A^2, E = k (r - r0)^2)
   and ``CHARMM_UREY_BRADLEY_EQUIL_VALUE`` (A).  Each term must join the ends of one of the
   file's angles.  The layout follows parmed's ``ChamberParm``; it is not pinned against an engine.
+* ``"gb"``: the Generalized Born ``RADII`` (A) and ``SCREEN`` sections, one value per atom, as ``gb_params``;
+  ``RADIUS_SET`` (e.g. "H(N)-modified Bondi radii (mbondi2)") is kept as ``AmberSystem.radius_set`` for the record.
 * ``"nbfix"``: LJ A/B over the type names from the full ``LENNARD_JONES_ACOEF/BCOEF`` through
   ``NONBONDED_PARM_INDEX`` (``TopologyParameters(nbfix=...)`` with sigma = (A/B)^(1/6),
   epsilon = B^2 / 4A per type pair), so that off-diagonal pair modifications (chamber NBFIX,
@@ -165,6 +167,14 @@ class AmberSystem:
                 raise ValueError(f"{prmtop_path}: CMAP_INDEX does not hold {nterm} terms on maps 1..{nmap}")
             self.cmap_idx, self.cmap_map = rows[:, :5], rows[:, 5]
 
+        # Generalized Born: intrinsic radii (A) and OBC screening factors, and the name of the radius set
+        self.gb_radius = np.array(p["RADII"], dtype=np.float64) if "RADII" in p else None
+        self.gb_screen = np.array(p["SCREEN"], dtype=np.float64) if "SCREEN" in p else None
+        self.radius_set = " ".join(p["RADIUS_SET"]).strip() if "RADIUS_SET" in p else None
+        for name, v in (("RADII", self.gb_radius), ("SCREEN", self.gb_screen)):
+            if v is not None and len(v) != self.natoms:
+                raise ValueError(f"{prmtop_path}: {name} holds {len(v)} values for {self.natoms} atoms")
+
         # chamber Urey-Bradley: term (i, k) -> type; type -> (k_ub, s0)
         self.ub_idx = np.zeros((0, 2), np.int64)
         self.ub_type = np.zeros(0, np.int64)
@@ -295,7 +305,9 @@ def amber_parameters(system, terms=None, precision=torch.float32, device="cpu"):
     ``Parameters(ParmedForcefield(mol, prmtop), mol, terms)`` (parameters.py:109-294).  ``"cmap"`` in ``terms``
     (not among the defaults) also builds the file's CMAP terms, ``"ureybradley"`` a chamber file's Urey-Bradley
     terms; without them they are left out with a warning.  ``"nbfix"`` takes the LJ tables from the file's full
-    ACOEF/BCOEF (module docstring)."""
+    ACOEF/BCOEF (module docstring).  ``"gb"`` sets ``gb_params`` from the file's ``RADII`` and ``SCREEN`` (the
+    Generalized Born radii and screening factors ``Forces(..., implicit_solvent="obc2")`` needs); a file without
+    them raises."""
     if terms is None:
         terms = ("bonds", "angles", "dihedrals", "impropers", "1-4", "lj")
     terms = [t.lower() for t in terms]
@@ -386,6 +398,12 @@ def amber_parameters(system, terms=None, precision=torch.float32, device="cpu"):
             warnings.warn(f"the topology has {len(system.ub_idx)} Urey-Bradley terms; they are left out unless terms includes "
                           "'ureybradley'", stacklevel=2)
     nbfix = system.nbfix_pairs(list(uq)) if "nbfix" in terms else None
+    gb = None
+    if "gb" in terms:
+        if system.gb_radius is None or system.gb_screen is None:
+            raise ValueError("'gb' needs the prmtop's RADII and SCREEN sections, and this file has no "
+                             + " and no ".join(n for n, v in (("RADII", system.gb_radius), ("SCREEN", system.gb_screen)) if v is None))
+        gb = (system.gb_radius, system.gb_screen)
     cmaps = None
     if len(system.cmap_idx):
         if "cmap" in terms:
@@ -407,6 +425,7 @@ def amber_parameters(system, terms=None, precision=torch.float32, device="cpu"):
         cmaps=cmaps,
         urey_bradley=urey_bradley,
         nbfix=nbfix,
+        gb=gb,
         precision=precision,
         device=device,
     )

@@ -115,6 +115,8 @@ class MonteCarloBarostat:
 
         if not isinstance(integ.forces, Forces) or integ.forces.external is not None:
             raise RuntimeError("MonteCarloBarostat needs a native torchmd_b200.Forces without an external plugin")
+        if integ.forces.implicit_solvent:
+            raise RuntimeError("MonteCarloBarostat needs a periodic box: implicit solvent runs without one")
         if not integ.T or integ.gamma is None:
             raise RuntimeError("MonteCarloBarostat needs a thermostat: give the Integrator T and gamma")
         self.kT = BOLTZMAN * (self.temperature if self.temperature is not None else float(integ.T))

@@ -26,6 +26,7 @@
 #include "double.cuh"
 #include "constrain.cuh"
 #include "pme.cuh"
+#include "gbsa.cuh"
 #include "barostat.cuh"
 #include "remd.cuh"
 
@@ -270,6 +271,15 @@ struct CtxPriv {
   const int* ladder = nullptr;
   double* remd_T = nullptr;
   double* remd_factor = nullptr;
+  // tmd_set_gb: OBC2 implicit solvent (gbsa.cuh); gb_radius empty means off.  Host tables (fp64), the kernels'
+  // arguments and their per-atom buffers (owned)
+  std::vector<double> gb_radius, gb_screen;
+  double gb_eps = 78.5, gb_sigma = 0.0;
+  GbArgs gb{};
+  double *gb_rho = nullptr, *gb_scr = nullptr, *gb_rad = nullptr, *gb_q = nullptr;
+  double *gb_born = nullptr, *gb_chain = nullptr, *gb_dedb = nullptr;
+  cudaStream_t gb_side = nullptr;  // fp32: the radii and energy passes run here, beside the pair kernel
+  cudaEvent_t gb_fork = nullptr, gb_join = nullptr;
 };
 
 }  // namespace
@@ -290,6 +300,7 @@ static int need_precision(tmd_ctx* ctx, int bits, const char* name) {
 
 // ---- particle-mesh Ewald: parameter choice (the one place it is made) ------------------------
 static inline bool pme_on(tmd_ctx* ctx) { return priv(ctx).pme_tol > 0.0; }
+static inline bool gb_on(tmd_ctx* ctx) { return !priv(ctx).gb_radius.empty(); }
 static int smallest_235(int n) {
   for (int m = std::max(n, 1);; ++m) {
     int k = m;
@@ -348,7 +359,7 @@ const char* tmd_last_error(void) { return g_err.c_str(); }
 #if defined(TMD_SIMT_HOST)
 int tmd_version(void) { return -100; }  // host SIMT interpreter build (tests/simt): torchmd_b200/_lib.py refuses it
 #else
-int tmd_version(void) { return 107; }  // 101: the "precision: double" entry points (tmd_set_precision, *_f64); 102: constraints; 103: PME; 104: box rescale + molecule scaling; 105: CMAP; 106: Urey-Bradley; 107: temperature ladder + replica exchange
+int tmd_version(void) { return 108; }  // 101: the "precision: double" entry points (tmd_set_precision, *_f64); 102: constraints; 103: PME; 104: box rescale + molecule scaling; 105: CMAP; 106: Urey-Bradley; 107: temperature ladder + replica exchange; 108: OBC2 implicit solvent
 #endif
 
 int tmd_create(tmd_ctx** out, int device, int natoms, int nreplicas) {
@@ -438,8 +449,12 @@ int tmd_destroy(tmd_ctx* ctx) {
     CtxPriv& p = priv(ctx);
     for (void* b : {(void*)p.pme_q, (void*)p.pme_L, (void*)p.pme_tw, (void*)p.pme_econst, (void*)p.pme_qgrid, p.pme_cgrid, p.pme_infl,
                     (void*)p.pme_mod, (void*)p.box_dev, (void*)p.mol_ptr, (void*)p.mol_atoms, (void*)p.mol_parent, (void*)p.mol_u,
-                    (void*)p.remd_T, (void*)p.remd_factor})
+                    (void*)p.remd_T, (void*)p.remd_factor, (void*)p.gb_rho, (void*)p.gb_scr, (void*)p.gb_rad, (void*)p.gb_q,
+                    (void*)p.gb_born, (void*)p.gb_chain, (void*)p.gb_dedb})
       if (b) cudaFree(b);
+    if (p.gb_side) cudaStreamDestroy(p.gb_side);
+    if (p.gb_fork) cudaEventDestroy(p.gb_fork);
+    if (p.gb_join) cudaEventDestroy(p.gb_join);
     if (p.pme_side) cudaStreamDestroy(p.pme_side);
     if (p.pme_fork) cudaEventDestroy(p.pme_fork);
     if (p.pme_join) cudaEventDestroy(p.pme_join);
@@ -873,6 +888,7 @@ int tmd_set_pme(tmd_ctx* ctx, double tolerance) {
   if (ctx->cutoff < 0) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_pme: particle-mesh Ewald needs a cutoff");
   if (ctx->rfa) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_pme: particle-mesh Ewald and the reaction field exclude each other");
   if (!(ctx->pair_mask & T_ELEC)) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_pme: particle-mesh Ewald needs the electrostatics term");
+  if (gb_on(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_pme: particle-mesh Ewald and implicit solvent exclude each other");
   if (ctx->have_box) {
     double alpha;
     int K[3];
@@ -894,6 +910,54 @@ int tmd_get_pme(tmd_ctx* ctx, double* alpha, int32_t grid[3]) {
   if (!ctx->have_box) return fail(TMD_ERR_STATE, "tmd_get_pme: the grid follows the box: call tmd_set_box first");
   *alpha = priv(ctx).pme_alpha;
   for (int d = 0; d < 3; ++d) grid[d] = priv(ctx).pme_K[d];
+  return TMD_OK;
+}
+
+// ---- OBC2 implicit solvent ----------------------------------------------------------------------
+// What GB cannot run with (gbsa.cuh sums every pair of a system without a box); "" when the context may use it.
+static const char* gb_conflict(tmd_ctx* ctx) {
+  if (ctx->dd_base || !ctx->d.own_all) return "decomposed runs cannot use implicit solvent";
+  if (pme_on(ctx)) return "particle-mesh Ewald and implicit solvent exclude each other";
+  if (ctx->have_nonbonded) {
+    if (!(ctx->pair_mask & T_ELEC)) return "implicit solvent needs the electrostatics term";
+    if (ctx->cutoff >= 0) return "implicit solvent sums every pair: it takes no cutoff";
+    if (ctx->rfa) return "implicit solvent and the reaction field exclude each other";
+  }
+  if (ctx->have_box && ctx->periodic) return "implicit solvent needs a system without a box (all box lengths zero)";
+  return "";
+}
+
+int tmd_set_gb(tmd_ctx* ctx, int n, const double* radius, const double* screen, double solvent_dielectric,
+               double surface_tension) {
+  if (!ctx || n < 0 || (n > 0 && (!radius || !screen))) return fail(TMD_ERR_ARG, "tmd_set_gb: bad arguments");
+  CtxPriv& pv = priv(ctx);
+  if (n == 0) {
+    if (gb_on(ctx)) {
+      pv.gb_radius.clear();
+      pv.gb_screen.clear();
+      pv.dirty = true;
+    }
+    return TMD_OK;
+  }
+  if (n != ctx->natoms) return fail(TMD_ERR_ARG, "tmd_set_gb: one radius and one screen per atom");
+  for (int i = 0; i < n; ++i) {
+    if (!(radius[i] > GB_OFFSET) || !std::isfinite(radius[i]))
+      return fail(TMD_ERR_ARG, "tmd_set_gb: radius of atom " + std::to_string(i) + " is not a finite value above 0.09 A");
+    if (!(screen[i] > 0.0) || !std::isfinite(screen[i]))
+      return fail(TMD_ERR_ARG, "tmd_set_gb: screen of atom " + std::to_string(i) + " is not a finite positive value");
+  }
+  if (!(solvent_dielectric > 0.0) || !std::isfinite(solvent_dielectric))
+    return fail(TMD_ERR_ARG, "tmd_set_gb: the solvent dielectric must be finite and positive");
+  if (!(surface_tension >= 0.0) || !std::isfinite(surface_tension))
+    return fail(TMD_ERR_ARG, "tmd_set_gb: the surface tension must be finite and not negative");
+  const char* why = gb_conflict(ctx);
+  if (*why) return fail(TMD_ERR_UNSUPPORTED, std::string("tmd_set_gb: ") + why);
+  pv.gb_radius.assign(radius, radius + n);
+  pv.gb_screen.assign(screen, screen + n);
+  pv.gb_eps = solvent_dielectric;
+  pv.gb_sigma = surface_tension;
+  ctx->touched = true;
+  pv.dirty = true;
   return TMD_OK;
 }
 
@@ -1039,6 +1103,46 @@ static int pme_finalize(tmd_ctx* ctx, cudaStream_t stream) {
   if (f64) launch_pme_influence<double>(ctx, stream);
   else launch_pme_influence<float>(ctx, stream);
   TMD_CUDA(cudaGetLastError());  // (set-up work: not counted with the force calls' launches)
+  return TMD_OK;
+}
+
+// OBC2 tables: rho = R - 0.09, S = screen rho, R, the scaled charges, and the per-replica radii, chain factors and dE/dB.
+static int gb_finalize(tmd_ctx* ctx) {
+  CtxPriv& pv = priv(ctx);
+  const char* why = gb_conflict(ctx);
+  if (*why) return fail(TMD_ERR_UNSUPPORTED, why);
+  const int N = ctx->natoms, R = ctx->nrep;
+  const bool f64 = ctx->precision == 64;
+  const double sk = sqrt(ctx->coulomb > 0 ? ctx->coulomb : 0.0);
+  std::vector<double> rho(N), scr(N), q(N);
+  for (int i = 0; i < N; ++i) {
+    rho[i] = pv.gb_radius[i] - GB_OFFSET;
+    scr[i] = pv.gb_screen[i] * rho[i];
+    q[i] = (f64 ? ctx->charges64_host[i] : (double)ctx->charges_host[i]) * sk;
+  }
+  int rc;
+  if ((rc = upload(&pv.gb_rho, rho.data(), rho.size()))) return rc;
+  if ((rc = upload(&pv.gb_scr, scr.data(), scr.size()))) return rc;
+  if ((rc = upload(&pv.gb_rad, pv.gb_radius.data(), pv.gb_radius.size()))) return rc;
+  if ((rc = upload(&pv.gb_q, q.data(), q.size()))) return rc;
+  for (double** b : {&pv.gb_born, &pv.gb_chain, &pv.gb_dedb})
+    if ((rc = device_alloc(b, (size_t)R * N))) return rc;
+  if (!f64 && !pv.gb_side) {
+    TMD_CUDA(cudaStreamCreateWithFlags(&pv.gb_side, cudaStreamNonBlocking));
+    TMD_CUDA(cudaEventCreateWithFlags(&pv.gb_fork, cudaEventDisableTiming));
+    TMD_CUDA(cudaEventCreateWithFlags(&pv.gb_join, cudaEventDisableTiming));
+  }
+  GbArgs& a = pv.gb;
+  a.natoms = N;
+  a.rho = pv.gb_rho;
+  a.scr = pv.gb_scr;
+  a.rad = pv.gb_rad;
+  a.q = pv.gb_q;
+  a.born = pv.gb_born;
+  a.chain = pv.gb_chain;
+  a.dedb = pv.gb_dedb;
+  a.pref = -(1.0 - 1.0 / pv.gb_eps);
+  a.np = 4.0 * M_PI * pv.gb_sigma;
   return TMD_OK;
 }
 
@@ -1473,6 +1577,7 @@ static int finalize(tmd_ctx* ctx, cudaStream_t stream) {
     D.pp.true_gradient = ctx->exact_gradient;
   }
   if (pme_on(ctx) && (rc = pme_finalize(ctx, stream))) return rc;
+  if (gb_on(ctx) && (rc = gb_finalize(ctx))) return rc;
   if (!priv(ctx).box_dev && (rc = device_alloc(&priv(ctx).box_dev, (size_t)R * 3))) return rc;
   TMD_CUDA(cudaMemcpy(priv(ctx).box_dev, ctx->box64_host.data(), (size_t)R * 3 * sizeof(double), cudaMemcpyHostToDevice));
   priv(ctx).grids = grids;
@@ -1682,6 +1787,23 @@ static int enqueue_pme_gather(tmd_ctx* ctx, const T* pos, T* forces, double* ene
   return TMD_OK;
 }
 
+// OBC2 (gbsa.cuh): the radii and energy passes need only the positions; k_gb_forces adds to complete pair forces.
+static inline dim3 gb_grid(const tmd_ctx* ctx) { return dim3((unsigned)((ctx->natoms + GB_WARPS - 1) / GB_WARPS), (unsigned)ctx->nrep); }
+template <typename T>
+static int enqueue_gb_radii_energy(tmd_ctx* ctx, const T* pos, double* energies, cudaStream_t s) {
+  launch(k_gb_radii<T>, gb_grid(ctx), GB_THREADS, s, priv(ctx).gb, pos);
+  TMD_LAUNCHED(ctx, "k_gb_radii");
+  launch(k_gb_energy<T>, gb_grid(ctx), GB_THREADS, s, priv(ctx).gb, pos, energies);
+  TMD_LAUNCHED(ctx, "k_gb_energy");
+  return TMD_OK;
+}
+template <typename T>
+static int enqueue_gb_forces(tmd_ctx* ctx, const T* pos, T* forces, cudaStream_t s) {
+  launch(k_gb_forces<T>, gb_grid(ctx), GB_THREADS, s, priv(ctx).gb, pos, forces);
+  TMD_LAUNCHED(ctx, "k_gb_forces");
+  return TMD_OK;
+}
+
 // Forces.compute on an fp64 context: preparation (fp32 shadow), the gated fp32 list build on the shadow, the fp64
 // records in the new order, k_pair_f64, then the two bonded passes in stream order.
 static int enqueue_forces_f64(tmd_ctx* ctx, const double* pos, double* forces, double* energies, cudaStream_t st) {
@@ -1702,6 +1824,10 @@ static int enqueue_forces_f64(tmd_ctx* ctx, const double* pos, double* forces, d
     if (int rc = enqueue_pair(ctx, pair_kernel_of(ctx), dim3((N + PAIR_WARPS - 1) / PAIR_WARPS, R), forces, energies, st)) return rc;
     if (pme)
       if (int rc = enqueue_pme_gather<double>(ctx, pos, forces, energies, st)) return rc;
+    if (gb_on(ctx)) {
+      if (int rc = enqueue_gb_radii_energy<double>(ctx, pos, energies, st)) return rc;
+      if (int rc = enqueue_gb_forces<double>(ctx, pos, forces, st)) return rc;
+    }
   } else {
     TMD_CUDA(cudaMemsetAsync(forces, 0, (size_t)R * N * 3 * sizeof(double), st));
   }
@@ -1769,6 +1895,15 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
     TMD_CUDA(cudaStreamWaitEvent(pv.pme_side, pv.pme_fork, 0));
     if (int prc = enqueue_pme_chain<float>(ctx, pos, energies, pv.pme_side)) return prc;
     TMD_CUDA(cudaEventRecord(pv.pme_join, pv.pme_side));
+  }
+  // implicit solvent: the radii and energy passes likewise, on their own stream; k_gb_forces joins after the pair kernel
+  const bool gb = gb_on(ctx);
+  if (gb) {
+    CtxPriv& pv = priv(ctx);
+    TMD_CUDA(cudaEventRecord(pv.gb_fork, st));
+    TMD_CUDA(cudaStreamWaitEvent(pv.gb_side, pv.gb_fork, 0));
+    if (int grc = enqueue_gb_radii_energy<float>(ctx, pos, energies, pv.gb_side)) return grc;
+    TMD_CUDA(cudaEventRecord(pv.gb_join, pv.gb_side));
   }
 
   BondedTablesT<float> T;
@@ -1865,6 +2000,10 @@ static int enqueue_forces(tmd_ctx* ctx, const float* pos, float* forces, double*
     if (pme) {
       TMD_CUDA(cudaStreamWaitEvent(st, pv.pme_join, 0));
       if (int prc = enqueue_pme_gather<float>(ctx, pos, forces, energies, st)) return prc;
+    }
+    if (gb) {
+      TMD_CUDA(cudaStreamWaitEvent(st, pv.gb_join, 0));
+      if (int grc = enqueue_gb_forces<float>(ctx, pos, forces, st)) return grc;
     }
   } else {
     TMD_CUDA(cudaMemsetAsync(forces, 0, (size_t)R * N * 3 * sizeof(float), st));
@@ -2368,6 +2507,7 @@ int tmd_set_owned_atoms(tmd_ctx* ctx, int first_atom, int count) {
   if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_owned_atoms: fp64 contexts run the whole system on one GPU");
   if (has_constraints(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_owned_atoms: a context with constraints runs the whole system on one GPU");
   if (pme_on(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_owned_atoms: a particle-mesh Ewald context runs the whole system on one GPU");
+  if (gb_on(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_set_owned_atoms: an implicit-solvent context runs the whole system on one GPU");
   ctx->d.own_lo = first_atom;
   ctx->d.own_n = count;
   ctx->d.own_all = (first_atom == 0 && count == ctx->natoms) ? 1 : 0;
@@ -2705,6 +2845,7 @@ int tmd_dd_create(tmd_ctx* ctx, int rank, int world, unsigned char* handle_out) 
   if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_create: fp64 contexts run the whole system on one GPU");
   if (has_constraints(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_create: a context with constraints runs the whole system on one GPU");
   if (pme_on(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_create: a particle-mesh Ewald context runs the whole system on one GPU");
+  if (gb_on(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_create: an implicit-solvent context runs the whole system on one GPU");
   if (ctx->nrep != 1) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_create: decomposed runs take one replica");
   static_assert(sizeof(cudaIpcMemHandle_t) == TMD_IPC_HANDLE_BYTES, "IPC handle size");
   DeviceGuard guard(ctx->device);
@@ -2730,6 +2871,7 @@ int tmd_dd_connect(tmd_ctx* ctx, const unsigned char* handles) {
   if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_connect: fp64 contexts run the whole system on one GPU");
   if (has_constraints(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_connect: a context with constraints runs the whole system on one GPU");
   if (pme_on(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_connect: a particle-mesh Ewald context runs the whole system on one GPU");
+  if (gb_on(ctx)) return fail(TMD_ERR_UNSUPPORTED, "tmd_dd_connect: an implicit-solvent context runs the whole system on one GPU");
   if (!ctx->dd_base) return fail(TMD_ERR_STATE, "tmd_dd_connect: tmd_dd_create has not been called");
   DeviceGuard guard(ctx->device);
   for (int p = 0; p < ctx->dd_world; ++p) {
@@ -2749,6 +2891,7 @@ int tmd_dd_connect(tmd_ctx* ctx, const unsigned char* handles) {
   if (ctx->precision == 64) return fail(TMD_ERR_UNSUPPORTED, name ": fp64 contexts run the whole system on one GPU"); \
   if (has_constraints(ctx)) return fail(TMD_ERR_UNSUPPORTED, name ": a context with constraints runs the whole system on one GPU"); \
   if (pme_on(ctx)) return fail(TMD_ERR_UNSUPPORTED, name ": a particle-mesh Ewald context runs the whole system on one GPU"); \
+  if (gb_on(ctx)) return fail(TMD_ERR_UNSUPPORTED, name ": an implicit-solvent context runs the whole system on one GPU"); \
   if (!ctx->dd_connected) return fail(TMD_ERR_STATE, name ": tmd_dd_create / tmd_dd_connect first"); \
   DeviceGuard guard(ctx->device);
 

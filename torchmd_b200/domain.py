@@ -96,6 +96,8 @@ class DecomposedIntegrator:
             raise NotImplementedError("per-replica temperatures run on one GPU: use Integrator(..., T=[...])")
         if getattr(forces, "pme", False):
             raise NotImplementedError("particle-mesh Ewald runs on one GPU: use Integrator with Forces(..., pme=True)")
+        if getattr(forces, "implicit_solvent", None):
+            raise NotImplementedError("implicit solvent runs on one GPU: use Integrator with Forces(..., implicit_solvent=...)")
         if system.pos.dtype == torch.float64:
             raise NotImplementedError("decomposed runs are fp32 only: run 'precision: double' on one GPU")
         if system.pos.shape[0] != 1:

@@ -60,7 +60,8 @@ class Forces:
         correction maps the parameters carry (``cmap_params``, built by the parameter builders when asked for
         ``"cmap"``); their energy is part of the ``dihedrals`` energy.  ``"angles"`` likewise turns on the Urey-Bradley
         1-3 terms the parameters carry (``ub_params``, built when asked for ``"ureybradley"``); their energy is part of
-        the ``angles`` energy.
+        the ``angles`` energy.  With ``implicit_solvent``, ``"electrostatics"`` also holds both Generalized Born
+        energies (polar and non-polar), as it holds PME's reciprocal energy.
     external : optional plugin exposing ``calculate(pos, box) -> (E (R,), F (R,N,3))``
     cutoff, rfa, solventDielectric, switch_dist, exclusions : as in the reference
     skin : Verlet-list buffer in Angstrom (not in the reference; results do not depend on it)
@@ -73,6 +74,14 @@ class Forces:
         crossing it changes the energy by k qi qj erfc(alpha rc) / rc: at the default 5e-4 an fp64 NVE run of rigid
         water at 2 fs keeps E_tot within 2.6 % of E_kin's fluctuation, at 1e-5 within 1.7 % (DESIGN.md 5b).  Runs
         that need tighter energy conservation should use a smaller tolerance.
+    implicit_solvent : ``"obc2"`` for Generalized Born implicit solvent (OBC2, AMBER igb=5; not in the reference), or
+        None.  Radii and screening factors come from ``parameters.gb_params`` (``amber_parameters(..., terms=[...,
+        "gb"])`` reads them from a prmtop); the solvent dielectric is ``solventDielectric``, the solute's 1.  The polar
+        energy -1/2 k (1 - 1/eps) sum_ij qi qj / f_GB over every pair (no exclusions, i = j included) and the
+        non-polar term are part of the ``electrostatics`` energy, and the forces are their exact gradient through
+        every Born radius.  Needs "electrostatics", no cutoff, no reaction field, no PME and an all-zero box.
+    surface_tension : sigma of the ACE non-polar term sum_i 4 pi sigma (R_i + 1.4)^2 (R_i / B_i)^6, kcal/mol/A^2
+        (OpenMM's default is 0.0054); 0 leaves it out, as AMBER's gbsa=0 does.
     """
 
     # 1-4 is listed with the bonded terms like in the reference (forces.py:22-25)
@@ -93,6 +102,8 @@ class Forces:
         skin=None,
         pme=False,
         ewald_tolerance=5e-4,
+        implicit_solvent=None,
+        surface_tension=0.0,
     ):
         self.par = parameters
         if terms is None:
@@ -121,6 +132,34 @@ class Forces:
                 raise RuntimeError("Particle-mesh Ewald and the reaction field approximation exclude each other")
             if not 0.0 < float(ewald_tolerance) < 0.5:
                 raise RuntimeError("ewald_tolerance must be between 0 and 0.5")
+        if implicit_solvent is not None:
+            if str(implicit_solvent).lower() != "obc2":
+                raise ValueError(f"implicit_solvent {implicit_solvent!r} is not implemented: 'obc2' or None")
+            implicit_solvent = "obc2"
+            if "electrostatics" not in self.energies:
+                raise RuntimeError("Implicit solvent needs the electrostatics term")
+            if cutoff is not None:
+                raise RuntimeError("Implicit solvent sums every pair: it takes no cutoff")
+            if rfa:
+                raise RuntimeError("Implicit solvent and the reaction field approximation exclude each other")
+            if pme:
+                raise RuntimeError("Implicit solvent and particle-mesh Ewald exclude each other")
+            if not (np.isfinite(float(surface_tension)) and float(surface_tension) >= 0.0):
+                raise RuntimeError("surface_tension must be finite and not negative (kcal/mol/A^2)")
+            if not (np.isfinite(float(solventDielectric)) and float(solventDielectric) > 0.0):
+                raise RuntimeError("Implicit solvent needs a finite positive solventDielectric")
+            gb = getattr(parameters, "gb_params", None)
+            if gb is None:
+                raise RuntimeError("Implicit solvent needs parameters.gb_params (amber_parameters(..., terms=[..., 'gb']))")
+            n = len(parameters.masses)
+            radius = np.asarray(gb["radius"].detach().cpu() if torch.is_tensor(gb["radius"]) else gb["radius"], np.float64).reshape(-1)
+            screen = np.asarray(gb["screen"].detach().cpu() if torch.is_tensor(gb["screen"]) else gb["screen"], np.float64).reshape(-1)
+            if len(radius) != n or len(screen) != n:
+                raise RuntimeError(f"gb_params must hold one radius and one screen per atom ({n})")
+            if not (np.isfinite(radius).all() and np.isfinite(screen).all()):
+                raise RuntimeError("gb_params holds a value that is not finite")
+            if (radius <= 0.09).any() or (screen <= 0).any():
+                raise RuntimeError("gb_params: every radius must be above 0.09 A and every screen positive")
 
         self.natoms = len(parameters.masses)
         self.require_distances = any(t in self.nonbonded for t in self.energies)
@@ -132,6 +171,8 @@ class Forces:
         self.skin = DEFAULT_SKIN if skin is None else float(skin)
         self.pme = bool(pme)
         self.ewald_tolerance = float(ewald_tolerance)
+        self.implicit_solvent = implicit_solvent
+        self.surface_tension = float(surface_tension)
         self._exclusion_types = tuple(exclusions)
         self._ava_idx = None
         self._ctx = None
@@ -251,6 +292,11 @@ class Forces:
         )
         if self.pme:
             check(L.tmd_set_pme(ctx, self.ewald_tolerance))
+        if self.implicit_solvent:
+            radius = _np(par.gb_params["radius"], np.float64)
+            screen = _np(par.gb_params["screen"], np.float64)
+            check(L.tmd_set_gb(ctx, self.natoms, _lib.ptr(radius), _lib.ptr(screen), float(self.solventDielectric),
+                               self.surface_tension))
 
         def instance_rows(term):
             """Per-instance parameter rows: params[map[:,1]] ordered by map[:,0]."""
@@ -301,6 +347,8 @@ class Forces:
             return
         f64 = self._ctx_key[2] == torch.float64
         diag = np.ascontiguousarray(torch.diagonal(box, dim1=1, dim2=2).detach().cpu().numpy().astype(np.float64 if f64 else np.float32))
+        if self.implicit_solvent and np.any(diag != 0):
+            raise RuntimeError("Implicit solvent needs a system without a box: every box length must be zero")
         L = _lib.lib()
         _lib.check((L.tmd_set_box_f64 if f64 else L.tmd_set_box)(self._ctx, _lib.ptr(diag)))
         self._box_key, self._box_ref = key, box

@@ -20,6 +20,10 @@ psi = dihedral(idx[t,1:5]) and map map_of[t]; map m holds E(phi_i, psi_j) at phi
 Urey-Bradley terms (not in the reference) are ``ub_params`` in the per-term layout with idx (U,3) = the angle
 (a, b, c) whose ends a, c the term joins and params (P,2) = k_ub [kcal/mol/A^2], s0 [A]; E = k_ub (r_ac - s0)^2.
 
+Generalized Born parameters (not in the reference) are ``gb_params = {"radius": (N,), "screen": (N,)}`` float64: the
+intrinsic radius R in A (a prmtop's RADII) and the OBC screening factor (SCREEN) of every atom; ``Forces(...,
+implicit_solvent="obc2")`` reads them.  They stay fp64 in both precisions.
+
 NBFIX pair overrides (not in the reference) are ``nbfix_params = {"idx": (P,2) int64 type pairs, "params": (P,2)
 sigma, epsilon}``: ``get_AB`` puts 4 eps sigma^12 and 4 eps sigma^6 at (t1, t2) and (t2, t1) of the Lorentz-Berthelot
 tables and leaves every other entry as it was.
@@ -96,6 +100,7 @@ class TopologyParameters:
         cmaps=None,
         urey_bradley=None,
         nbfix=None,
+        gb=None,
         precision=torch.float32,
         device="cpu",
     ):
@@ -108,6 +113,7 @@ class TopologyParameters:
         cmaps : optional ``(idx (n,5), map_of (n,), res (nmaps,), grids)`` CMAP terms and maps (module docstring)
         urey_bradley : optional ``(idx (U,3) angle triples, map, params (P,2) = k_ub, s0)`` (module docstring)
         nbfix : optional ``(type pairs (P,2), params (P,2) = sigma, epsilon)`` LJ overrides applied by ``get_AB``
+        gb : optional ``(radius (N,), screen (N,))`` Generalized Born parameters (module docstring)
         """
         self.natoms = int(len(atom_types))
         self.mapped_atom_types = torch.as_tensor(
@@ -136,6 +142,12 @@ class TopologyParameters:
         if self.ub_params is not None and (int(self.ub_params["idx"].min()) < 0 or int(self.ub_params["idx"].max()) >= self.natoms):
             raise ValueError("urey_bradley: atom index out of range")
         self.nbfix_params = _nbfix(*nbfix, len(nb)) if nbfix is not None and len(nbfix[0]) else None
+        self.gb_params = None
+        if gb is not None:
+            radius, screen = (torch.as_tensor(np.asarray(v, dtype=np.float64).reshape(-1)) for v in gb)
+            if len(radius) != self.natoms or len(screen) != self.natoms:
+                raise ValueError("gb: one radius and one screen per atom")
+            self.gb_params = {"radius": radius, "screen": screen}
         self.A = None
         self.B = None
         self.device = "cpu"
@@ -165,6 +177,8 @@ class TopologyParameters:
                     t[k] = t[k].to(device)
         if self.cmap_params is not None:
             self.cmap_params = {k: v.to(device) for k, v in self.cmap_params.items()}
+        if self.gb_params is not None:
+            self.gb_params = {k: v.to(device) for k, v in self.gb_params.items()}
         if self.A is not None:
             self.A, self.B = self.A.to(device), self.B.to(device)
         self.device = device
